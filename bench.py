@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the DiffSBDD denoising hot path on B200 (BASELINE.json metric).
+"""Benchmark of the DiffSBDD denoising hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-gpu]
-                    [--workload fullatom|ca|inpaint]
+                    [--workload fullatom|ca|inpaint] [--dump-outputs DIR]
 
 metric : ligand atoms/s through the full DDPM sampling loop of the per-GPU batch.
 workload (BASELINE.json configs, SURVEY.md §8(d)):
@@ -15,10 +15,14 @@ step   : ONE complete sampling run (``sample_given_pocket`` / ``inpaint``) of th
 value  : whole-job atoms/s with the inputs already resident in HBM (CUDA events, max over ranks).
 e2e    : same metric through the public API from pinned HOST buffers, host->device copies of the inputs and the
          device->host read of the ligands inside the timed region.
---impl reference     : the reference's CPU implementation of the path (oracle port — /root/reference cannot travel to the
-                       GPU box), all host threads it can use, bounded sample per step, extrapolated linearly.
---impl reference-gpu : the same ATen op sequence as the reference on the B200 (device='cuda', eager, reference-order DDPM
+--impl b200          : this project's native kernels (the arm keeps its historical name; they are built for sm_90a).
+--impl reference     : the reference's CPU implementation of the path (the oracle port of its op sequence), all host
+                       threads it can use, bounded sample per step, extrapolated linearly.
+--impl reference-gpu : the same ATen op sequence as the reference on the GPU (device='cuda', eager, reference-order DDPM
                        loop): the fair "beat this" number of SURVEY.md §8(d); bounded sample, extrapolated linearly.
+--dump-outputs DIR   : (native arm) after the timed steps, writes what the last timed step returned to its caller as
+                       DIR/<name>.npy (float32 / float64).  The inputs and seeds depend only on the arguments, so two builds
+                       run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -72,6 +76,8 @@ def parse_args():
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--profile-calls', type=int, default=10)
     ap.add_argument('--cpu-sample-seconds', type=float, default=20.0)
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the arrays the last timed step returned as DIR/<name>.npy')
     args = ap.parse_args()
     _, b, nl, npk, _, _, _, _ = WORKLOADS[args.workload]
     args.batch = b if args.batch is None else args.batch
@@ -115,11 +121,11 @@ def workload_config(args, world=1):
     if args.workload == 'inpaint':
         cfg.update({'inpaint_timesteps': args.inpaint_timesteps, 'resamplings': args.resamplings, 'n_fixed': args.n_fixed,
                     'center': 'ligand'})
-    # the same text in every arm (the driver compares the `config` objects of the arms); what differs per arm is in `arm`
+    # the same text in every arm (so that the `config` objects of the arms compare equal); what differs per arm is in `arm`
     cfg.update({'weights': 'synthetic seed 0 (diffsbdd_b200/synthetic.py), random-init of the named architecture',
                 'parallelism': (f'dp{world}: contiguous pocket shards per rank (diffsbdd_b200.distributed), no collective inside the '
                                 'loop, final all_gather of the ligands; the reference arm runs on rank 0 only'),
-                'l2': ('b200 arm: 256 MiB read+write flush before every timed step and e2e step; reference arms: none '
+                'l2': ('native arm: 256 MiB read+write flush before every timed step and e2e step; reference arms: none '
                        '(CPU arm / eager GPU arm whose working set exceeds L2 per call)')})
     return cfg
 
@@ -157,7 +163,7 @@ def inpaint_inputs(cfg, args, n_graphs, seed, device='cpu'):
     return {k: v.to(device) for k, v in lig.items()}, fixed.to(device)
 
 
-# ---- clocks sampler (B200_PROFILING.md "clocks DURING the timed region") -------------------------------------
+# ---- clocks sampler: SM clock, power and throttle reasons DURING the timed region -----------------------------------
 class ClockSampler:
     FIELDS = ('uuid,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,'
               'clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,'
@@ -212,8 +218,36 @@ class ClockSampler:
                 'power_w_max': max(power) if power else None, 'samples': len(sm), 'reasons': sorted(reasons)}
 
 
+def power_limit_w():
+    """Enforced power limit of GPU 0 as nvidia-smi reports it (None when unavailable): part of every number measured."""
+    try:
+        out = subprocess.run(['nvidia-smi', '--id=0', '--query-gpu=power.limit', '--format=csv,noheader,nounits'],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        return float(out.splitlines()[0])
+    except Exception:
+        return None
+
+
+def dump_outputs(out_dir, arrays, max_bytes=64 << 20):
+    """Writes every tensor of `arrays` as out_dir/<name>.npy: floating point as float32, integers as float64 (exact).
+    An array that would push the total past max_bytes is replaced by a fixed, seeded sample of its rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, t in sorted(arrays.items()):
+        a = t.detach().cpu()
+        a = a.float().numpy() if a.is_floating_point() else a.double().numpy()
+        if total + a.nbytes > max_bytes:
+            keep = int(a.shape[0] * (max_bytes - total) / a.nbytes) if a.ndim > 0 else 0
+            if keep <= 0:                      # budget spent: the array is left out
+                continue
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=min(keep, a.shape[0]), replace=False))
+            a = a[rows]
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
+        total += a.nbytes
+
+
 def l2_flush(buf):
-    buf.add_(1.0)    # read+write 256 MiB > 126 MB L2
+    buf.add_(1.0)    # read+write 256 MiB > 50 MB L2 of the H100
 
 
 # ---- reference arms: the oracle port of the reference's PyTorch path, on the host cores or eager on the GPU -----------
@@ -333,7 +367,7 @@ def run_reference(args):
 
 
 def run_reference_gpu(args):
-    """The reference's op sequence (oracle port, device='cuda') inside the reference-order eager loop on ONE B200, full
+    """The reference's op sequence (oracle port, device='cuda') inside the reference-order eager loop on ONE GPU, full
     batch: ``sub`` reverse steps + the final call per timed step, extrapolated to the full loop."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
@@ -345,12 +379,12 @@ def run_reference_gpu(args):
     ddpm, dyn, cfg, density = _reference_ddpm(args, device)
     sub = 20
     torch.manual_seed(0)
-    for _ in range(max(1, min(args.warmup, 2))):
+    for _ in range(args.warmup):
         _reference_run(args, ddpm, cfg, density, args.batch, 2, device)
     dyn.calls = 0
     sampler = ClockSampler(torch.device(device))
     sampler.start()
-    times = [_reference_run(args, ddpm, cfg, density, args.batch, sub, device) for _ in range(max(1, min(args.steps, 5)))]
+    times = [_reference_run(args, ddpm, cfg, density, args.batch, sub, device) for _ in range(args.steps)]
     clocks = sampler.stop()
     per_call = sum(times) / dyn.calls
     n_calls = denoiser_calls(args)
@@ -367,7 +401,7 @@ def run_reference_gpu(args):
     print(json.dumps(line), flush=True)
 
 
-# ---- B200 arm ---------------------------------------------------------------------------------------------------
+# ---- native arm -------------------------------------------------------------------------------------------------
 def run_b200(args):
     import torch.distributed as dist
     from diffsbdd_b200 import synthetic as syn
@@ -425,12 +459,15 @@ def run_b200(args):
     def step_device():
         step_no[0] += 1
         if inpaint:
-            xh_lig, _, _, _ = ddpm.inpaint({k: v.clone() for k, v in lig_dev.items()}, dict(pocket_dev), fixed_dev,
-                                           resamplings=args.resamplings, timesteps=args.inpaint_timesteps, center='ligand')
-            return xh_lig
+            xh_lig, xh_pocket, lig_mask, pocket_mask = ddpm.inpaint(
+                {k: v.clone() for k, v in lig_dev.items()}, dict(pocket_dev), fixed_dev,
+                resamplings=args.resamplings, timesteps=args.inpaint_timesteps, center='ligand')
+            return {'xh_lig': xh_lig, 'xh_pocket': xh_pocket, 'lig_mask': lig_mask, 'pocket_mask': pocket_mask}
         # library path: this rank's shard + the final all_gather of the ligands (the only collective of the path)
-        xh_all, _, _ = sample_given_pocket_sharded(ddpm, dict(job_dev), n_lig_job, base_seed=1000 * step_no[0], timesteps=T)
-        return xh_all
+        xh_all, sizes_all, local = sample_given_pocket_sharded(ddpm, dict(job_dev), n_lig_job, base_seed=1000 * step_no[0],
+                                                               timesteps=T)
+        return {'xh_lig_all': xh_all, 'lig_sizes_all': sizes_all, 'xh_lig': local[0], 'xh_pocket': local[1],
+                'lig_mask': local[2], 'pocket_mask': local[3]}
 
     def step_e2e():
         pocket = {k: v.to(device, non_blocking=True) for k, v in pocket_host.items()}
@@ -444,14 +481,17 @@ def run_b200(args):
             xh_lig, _, lig_mask, _ = model.generate_ligand_tensors(pocket, n_lig, timesteps=T)
         return xh_lig.cpu(), lig_mask.cpu()
 
+    last = {}
+
     def timed(fn, k):
-        """k steps between two events; returns (max over ranks of the total ms, per-rank total ms list)."""
+        """k steps between two events; returns (max over ranks of the total ms, per-rank total ms list).  The last step's
+        return value is kept in `last`."""
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(k):
             l2_flush(flush_buf)
-            fn()
+            last['out'] = fn()
         e1.record()
         torch.cuda.synchronize(device)
         ms = torch.tensor([e0.elapsed_time(e1)], device=device)
@@ -469,6 +509,8 @@ def run_b200(args):
     sampler.start()
     ms_total, per_rank_ms = timed(step_device, args.steps)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['out'])
     clocks_by_rank = None
     if world > 1:      # every rank sampled its own GPU: the per-rank clocks / power / throttle reasons name the limiter of a slow rank
         allc = [None] * world
@@ -530,35 +572,14 @@ def run_b200(args):
             # (+SiLU), the HxH second layer, SiLU, attention gate and the receiver segment sum
             alg_bytes = N * 2 * H * 4 + N * H * 4 + E * 12 + N * 16 + (H * H + 7 * H) * 4
             alg_flops = E * (2 * H * H + 12 * H)
-            peaks = {}
-            try:
-                with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
-                    peaks = json.load(f)
-            except Exception:
-                pass
-            hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-            tens_peak = float(peaks.get('bf16_tflops', 1590.0))
-            src = 'MEASURED_PEAKS.json (of measured)' if peaks else 'B200_PROFILING.md fallback (of fallback)'
-            traffic, traffic_src, traffic_edges = None, None, None
-            try:   # DRAM bytes per launch from the committed ncu --set full capture (never measured under the profiler here)
-                with open(os.path.join(ROOT, 'profiles', 'roofline_traffic.json')) as f:
-                    tj = json.load(f)
-                # the capture is of the full-atom dimensions (N = 64 x 200 nodes); inpaint runs the same shapes, other workloads have none
-                tr = tj.get(f'{kname}@{args.workload}') or (tj.get(kname) if args.workload in ('fullatom', 'inpaint') else None)
-                if tr:
-                    traffic, traffic_src, traffic_edges = tr['dram_bytes_per_launch'], tr['source'], tr.get('edges')
-            except Exception:
-                pass
+            # NVIDIA H100 SXM data sheet (dense, 700 W card): 3.35 TB/s HBM3, 989 TFLOP/s BF16 -- not a measured rate
+            hbm_peak, tens_peak = 3350.0, 989.0
+            src = 'H100 SXM data sheet'
             ach_b = alg_bytes / (gcl_ms * 1e-3) / 1e9
             ach_f = alg_flops / (gcl_ms * 1e-3) / 1e12
-            smax = (clocks.get('sm_max_mhz') or 1965.0)
+            smax = (clocks.get('sm_max_mhz') or 1980.0)
             fp32_peak = torch.cuda.get_device_properties(device).multi_processor_count * 128 * 2 * smax * 1e6 / 1e12
-            # the capture's geometry has more edges than this launch: only the 12 B/edge of CSR indices and input distances scale with E
-            if traffic is not None and traffic_edges:
-                traffic = int(traffic - 12 * (traffic_edges - E))
-                traffic_src += f'; captured at E={traffic_edges}, reported for E={E} (-12 B per edge)'
-            common = {'kernel': kname, 'avg_launch_ms': gcl_ms, 'edges': E, 'traffic': traffic, 'traffic_edges': traffic_edges,
-                      'traffic_source': traffic_src, 'algorithmic_bytes_per_launch': alg_bytes,
+            common = {'kernel': kname, 'avg_launch_ms': gcl_ms, 'edges': E, 'algorithmic_bytes_per_launch': alg_bytes,
                       'algorithmic_flops_per_launch': alg_flops}
             if tensor_path:
                 # the contraction runs on the tensor pipe as 3 split products: executed tensor FLOPs = 3 x algorithmic
@@ -589,9 +610,10 @@ def run_b200(args):
         if ddpm._graph_cache:
             engine = ('cuda_graph replay: denoiser + fused reverse update + fused RePaint iteration per (s, u)' if inpaint
                       else 'cuda_graph replay of one reverse step')
-        arm = {'what': 'diffsbdd_b200 (sm_100a kernels through the C ABI)',
-               'arithmetic': {0: 'fp32 FFMA', 7: '3xTF32 tcgen05', 15: '3xFP16 tcgen05'}.get(dyn.math_mode, str(dyn.math_mode)),
-               'edges_last_call': e_last, 'loop_engine': engine}
+        arm = {'what': 'diffsbdd_b200 (sm_90a kernels through the C ABI)',
+               'arithmetic': {0: 'fp32 FFMA', 7: '3xTF32 wgmma', 15: '3xFP16 wgmma'}.get(dyn.math_mode, str(dyn.math_mode)),
+               'edges_last_call': e_last, 'loop_engine': engine, 'gpu': torch.cuda.get_device_name(device),
+               'power_limit_w': power_limit_w()}
         per_rank_step = [m / args.steps for m in per_rank_ms]
         line = {'arm': arm, 'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps,
                 'warmup': args.warmup, 'ms_per_step': ms_total / args.steps, 'higher_is_better': True,

@@ -16,8 +16,8 @@ _LIB: Optional[C.CDLL] = None
 EXPORTED_SYMBOLS = (
     'dsb_param_count', 'dsb_param_name', 'dsb_dynamics_create', 'dsb_dynamics_destroy',
     'dsb_edge_capacity', 'dsb_dynamics_workspace_bytes', 'dsb_dynamics_forward', 'dsb_dynamics_edges',
-    'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_set_kernel_variants', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
-    'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_last_error', 'dsb_version', 'dsb_debug_set_tc_flags', 'dsb_debug_read_tc_prof',
+    'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
+    'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_last_error', 'dsb_version',
 )
 
 
@@ -49,19 +49,17 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     global _LIB
     if _LIB is not None:
         return _LIB
-    instr = os.environ.get('DSB_INSTRUMENT', '0') not in ('', '0')      # profiling tools only (profiles/tc_ablate.py)
-    path = _build.INSTR_LIB_PATH if instr else _build.LIB_PATH
-    if os.environ.get('DSB_LIB_PATH'):                                  # tuning builds (profiles/build_variants.py)
+    path = _build.LIB_PATH
+    if os.environ.get('DSB_LIB_PATH'):                                  # a library built elsewhere (e.g. with other flags)
         path = os.environ['DSB_LIB_PATH']
-    if os.environ.get('DSB_LIB_PATH'):
         if not os.path.exists(path):
             raise NativeError(f'DSB_LIB_PATH={path} does not exist')
-    elif not os.path.exists(path) or not _build.is_current(instrumented=instr):
+    elif not os.path.exists(path) or not _build.is_current():
         # missing, or built from other sources than the ones next to it (the .so is git-ignored and travels separately):
         # a stale library behind fixed ctypes signatures would corrupt memory silently
         if not build_if_missing:
             raise NativeError(f'{path} is missing or stale: run `python -m diffsbdd_b200._build` (needs nvcc)')
-        _build.build(instrumented=instr)
+        _build.build()
     lib = C.CDLL(path)
     vp, i64, i32 = C.c_void_p, C.c_int64, C.c_int32
     lib.dsb_last_error.restype = C.c_char_p
@@ -87,8 +85,6 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dsb_dynamics_last_launch_count.restype = C.c_int
     lib.dsb_set_programmatic_launch.argtypes = [C.c_int]
     lib.dsb_set_programmatic_launch.restype = C.c_int
-    lib.dsb_set_kernel_variants.argtypes = [C.c_int]
-    lib.dsb_set_kernel_variants.restype = C.c_int
     lib.dsb_dynamics_set_math_mode.argtypes = [vp, C.c_int]
     lib.dsb_dynamics_set_math_mode.restype = C.c_int
     lib.dsb_dynamics_set_profiling.argtypes = [vp, C.c_int]

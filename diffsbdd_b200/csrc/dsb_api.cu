@@ -645,7 +645,7 @@ using namespace dsb;
 extern "C" {
 
 const char* dsb_last_error(void) { return g_err; }
-const char* dsb_version(void) { return "diffsbdd_b200 0.3 (sm_100a: tcgen05 3xFP16 CTA-pair edge kernels and fused node block kernel, 3xTF32 single-CTA kernels, fp32 FFMA kernels)"; }
+const char* dsb_version(void) { return "diffsbdd_b200 0.4 (sm_90a: wgmma 3xFP16 / 3xTF32 edge and node GEMM kernels, fp32 FFMA kernels)"; }
 
 int dsb_param_count(const dsb_config* cfg) {
   if (int e = validate(cfg)) return e;
@@ -810,9 +810,7 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
   const int nq = nm * 2 * H, ldP = nq + 2 * H, nrecv = nm * H;
   const PView pv_gcl = {ws.P + nq, ldP}, pv_coord = {ws.P, ldP};
   const bool conditional = dm.n_coord_rows < dm.N;
-  static const bool no_fused_mlp = getenv("DSB_NO_FUSED_MLP") != nullptr;      // A/B timing switch (two node GEMMs instead)
   for (int l = 0; l < c.n_layers; ++l) {
-    bool fused_block = false;
     for (int sub = 0; sub < c.inv_sublayers; ++sub) {
       const GclW& G = dyn->w.gcl[l][sub];
       if (!(sub == 0 && l > 0)) {      // otherwise produced by the previous block's merged GEMM
@@ -825,40 +823,27 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
       DSB_TRY((mm & 2) ? launch_tc_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, f16, status, s) : launch_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, s));
       // node_model: h + W4 SiLU(W3 [h | agg/norm] + b3) + b4   (egnn_new.py:48-58)
       mark(KC_NODE_GEMM);
-      const EquivW& Qb = dyn->w.eq[l];
-      if ((mm & 1) && sub == c.inv_sublayers - 1 && G.iW3.h_hi && G.iW4.h_hi && Qb.iW1.h_hi && !no_fused_mlp && tc_node_block_available(H, f16)) {
-        // node_model and the merged first-layer GEMM of this block in one CTA-pair kernel (h converted to operand format once)
-        DSB_TRY(launch_tc_node_block(dyn, dm, ws, G, Qb, ws.P, ldP, conditional ? dm.n_coord_rows : 0, conditional ? nrecv : 0, s));
-        launches += 2 + ((g_kernel_variants & 4) ? 1 : 0);      // GCL edge kernel + block kernel (+ the split-off GEMM)
-        fused_block = true;
-      } else if ((mm & 1) && G.iW3.t_hi && G.iW4.t_hi && !no_fused_mlp) {
-        DSB_TRY(launch_tc_node_mlp(dyn, dm, ws, G, f16, status, s));        // both layers in one kernel, hidden stays on chip
-        launches += 2;
-      } else {
-        GemmArgs g2 = {ws.h, H, H, ws.agg, H, H, c.normalization_factor, G.W3, H, G.b3, nullptr, 0, ws.hT, H, dm.N, H, 1, nullptr, 0, 0, 0,
-                       c.aggregation_mean ? ws.deg : nullptr};
-        DSB_TRY(gemm(g2, G.iW3));
-        GemmArgs g3 = {ws.hT, H, H, nullptr, 0, 0, 1.f, G.W4, H, G.b4, ws.h, H, ws.h, H, dm.N, H, 0, ws.agg, H, 0, 0};
-        DSB_TRY(gemm(g3, G.iW4));
-        launches += 3;
-      }
+      GemmArgs g2 = {ws.h, H, H, ws.agg, H, H, c.normalization_factor, G.W3, H, G.b3, nullptr, 0, ws.hT, H, dm.N, H, 1, nullptr, 0, 0, 0,
+                     c.aggregation_mean ? ws.deg : nullptr};
+      DSB_TRY(gemm(g2, G.iW3));
+      GemmArgs g3 = {ws.hT, H, H, nullptr, 0, 0, 1.f, G.W4, H, G.b4, ws.h, H, ws.h, H, dm.N, H, 0, ws.agg, H, 0, 0};
+      DSB_TRY(gemm(g3, G.iW4));
+      launches += 3;      // edge kernel, two node GEMMs
     }
     // one GEMM for everything that consumes the updated h: this block's coord/cross first layers and the next block's
     // edge first layer.  In conditional mode the receiver-side coord columns are needed for ligand rows only.
     const EquivW& Q = dyn->w.eq[l];
     mark(KC_NODE_GEMM);
-    if (!fused_block) {
     GemmArgs g4 = {ws.h, H, H, nullptr, 0, 0, 1.f, Q.W1, Q.nq + Q.np, Q.b1, nullptr, 0, ws.P, ldP, dm.N, Q.nq + Q.np, 0, nullptr, 0,
                    conditional ? dm.n_coord_rows : 0, conditional ? nrecv : 0};
     DSB_TRY(gemm(g4, Q.iW1));
-    }
     mark(KC_EDGE_COORD);
     DSB_TRY((mm & 4) ? launch_tc_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, f16, status, s) : launch_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, s));
     float4* xnext = ws.xbuf[1 + (l & 1)];
     mark(KC_COORD_FINISH);
     DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, xnext, true, s));
     xcur = xnext;
-    launches += fused_block ? 2 : 3;      // (merged GEMM,) coordinate edge kernel, finish
+    launches += 3;      // merged GEMM, coordinate edge kernel, finish
   }
   mark(KC_POST);
   DSB_TRY(launch_post(dyn, dm, ws, xcur, out_atoms, out_residues, status, s));
@@ -876,17 +861,11 @@ int dsb_set_programmatic_launch(int enable) {
   return old;
 }
 
-int dsb_set_kernel_variants(int variants) {
-  const int old = dsb::g_kernel_variants;
-  if (variants >= 0) dsb::g_kernel_variants = variants & 7;
-  return old;
-}
-
 int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode) {
   if (!dyn) { set_error("null handle"); return DSB_ERR_INVALID_ARGUMENT; }
   if (mode < 0 || mode > 15) { set_error("math mode must be a bitmask in [0,15]"); return DSB_ERR_INVALID_ARGUMENT; }
   if (mode != 0 && dyn->cfg.sin_embedding) { set_error("sin_embedding is built in the fp32 FFMA kernels only (math mode 0)"); return DSB_ERR_UNSUPPORTED_CONFIG; }
-  if (mode != 0 && !tc_width_supported(dyn->cfg.hidden_nf)) { set_error("the tcgen05 kernels are built for hidden_nf 128, 192 and 256 only"); return DSB_ERR_UNSUPPORTED_CONFIG; }
+  if (mode != 0 && !tc_width_supported(dyn->cfg.hidden_nf)) { set_error("the tensor-core kernels are built for hidden_nf 128, 192 and 256 only"); return DSB_ERR_UNSUPPORTED_CONFIG; }
   dyn->math_mode = mode;
   return 0;
 }

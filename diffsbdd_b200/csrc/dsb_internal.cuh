@@ -1,4 +1,4 @@
-// Internal declarations shared by the translation units of libdiffsbdd_b200.so (sm_100a only).
+// Internal declarations shared by the translation units of libdiffsbdd_b200.so (sm_90a only).
 #pragma once
 #include <cstring>
 
@@ -112,8 +112,8 @@ struct dsb_dynamics {
   dsb::PackedWeights w;
   float* blob = nullptr;
   size_t blob_floats = 0;
-  int num_sms = 148;
-  int math_mode = 0;         // bitmask: 1 node GEMMs, 2 edge_gcl, 4 edge_coord on tcgen05 (H in {128,192,256}); 8: 3xFP16 split instead of 3xTF32
+  int num_sms = 132;
+  int math_mode = 0;         // bitmask: 1 node GEMMs, 2 edge_gcl, 4 edge_coord on wgmma (H in {128,192,256}); 8: 3xFP16 split instead of 3xTF32
   int last_launches = 0;     // kernels only
   int last_memsets = 0;
   // profiling
@@ -142,10 +142,9 @@ void set_error(const char* fmt, ...);
 // With g_pdl != 0 the forward's kernels are launched with cudaLaunchAttributeProgrammaticStreamSerialization:
 // every such kernel triggers its dependents at entry (pdl_trigger) and executes griddepcontrol.wait (pdl_wait)
 // before its first access to global memory a predecessor may have touched, so a kernel's launch latency and
-// prologue (barrier init, TMEM allocation, constant-vector staging) overlap the predecessor's tail.  Both
+// prologue (barrier init, constant-vector staging) overlap the predecessor's tail.  Both
 // instructions are no-ops for a kernel launched without the attribute.
 extern int g_pdl;
-extern int g_kernel_variants;      // dsb_set_kernel_variants (dsb_tc.cu)
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
   cudaLaunchConfig_t cfg = {};
@@ -155,22 +154,6 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-  }
-  return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
-// the same for a kernel that runs as clusters of two CTAs (CTA pairs on one TPC: tcgen05 cta_group::2); grid must be even
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k_pair(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  if (g_pdl) {
-    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 2;
   }
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
@@ -222,10 +205,6 @@ int configure_tc_kernels(int H);
 bool tc_width_supported(int H);     // hidden_nf values with tensor-core kernels (128, 192, 256)
 int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage& w, int n_tile_off, bool f16, int32_t* status,
                         cudaStream_t s);
-int launch_tc_node_mlp(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, bool f16, int32_t* status, cudaStream_t s);
-bool tc_node_block_available(int H, bool f16);
-int launch_tc_node_block(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const EquivW& q, float* P, int ldp,
-                         int dead_rows_from, int dead_cols, cudaStream_t s);
 int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const float4* x, PView pv, bool f16,
                        int32_t* status, cudaStream_t s);
 int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w, const float4* x, PView pv, bool f16,
@@ -242,14 +221,13 @@ __device__ __forceinline__ float silu_f(float x) { return x * rcp_approx(1.0f + 
 __device__ __forceinline__ float sigmoid_f(float x) { return rcp_approx(1.0f + ex2_approx(x * -1.4426950408889634f)); }
 
 
-// Packed fp32x2 arithmetic (FFMA2 / FADD2 / FMUL2 on sm_100a): the same IEEE operations as two scalar instructions, one
-// issue slot.  A pair is carried in a 64-bit register pair (u64); scalar operands broadcast for free in SASS.
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float a, float b) { f32x2 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { f32x2 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+// fp32 pairs: the tensor-core kernels handle activations four at a time as two pairs (one scalar instruction per element)
+typedef float2 f32x2;
+__device__ __forceinline__ f32x2 pk2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void upk2(f32x2 v, float& a, float& b) { a = v.x; b = v.y; }
+__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 // silu_f on a pair: bit-identical to two silu_f calls (same operations in the same order)
 __device__ __forceinline__ f32x2 silu2(f32x2 u) {
   float a, b;
@@ -258,8 +236,8 @@ __device__ __forceinline__ f32x2 silu2(f32x2 u) {
   return mul2(u, pk2(rcp_approx(a), rcp_approx(b)));
 }
 
-// SiLU of four values with TWO reciprocals instead of four: the 16-lane XU pipe (MUFU: 8 issue cycles per warp instruction
-// and sub-partition) is the busiest pipe of the edge kernels (2 SiLU per edge element = 4 MUFU), the FMA pipe is not.
+// SiLU of four values with TWO reciprocals instead of four: the 16-lane MUFU pipe is the busiest pipe of the edge kernels
+// (2 SiLU per edge element = 4 MUFU), the FMA pipe is not.
 //   d_i = 1 + 2^{t_i},  r = 1 / (d_a d_b)  ->  1/d_a = r d_b,  1/d_b = r d_a          (elements 0,2 and 1,3 are paired)
 // The exponent argument is clamped to 64 (pre-activation >= -44.4, where SiLU(x) = x e^x is below 3e-18 in magnitude) so that
 // neither d nor, harmfully, the product can reach inf next to a finite partner (0 * inf); a product of exactly 2^128 gives

@@ -1,54 +1,53 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX wrappers and the shared pipeline pieces of the tensor-core path.
+// wgmma / mbarrier / bulk-copy PTX wrappers and the operand-format helpers of the tensor-core path (sm_90a).
 //
-// Numerics: every contraction is a 3-product split accumulated in fp32 inside TMEM, in one of two operand formats:
-//   3xTF32 (kind::tf32, 4 B/operand element, 8-bit exponent: range-robust), or
-//   3xFP16 (kind::f16,  2 B/operand element: half the shared-memory operand traffic and twice the MMA rate; operands are
+// Numerics: every contraction is a 3-product split accumulated in fp32 registers by wgmma, in one of two operand formats:
+//   3xTF32 (tf32 operands, 4 B/operand element, 8-bit exponent: range-robust), or
+//   3xFP16 (f16 operands,  2 B/operand element: half the shared-memory operand traffic and twice the MMA rate; operands are
 //           pre-scaled by powers of two so residuals stay in fp16's normal range; |x| > 65504 -> inf -> NaN flag of the output).
 // 3xTF32:
 //     a = a_hi + a_lo,  a_hi = cvt.rna.tf32(a),  a_lo = a - a_hi   (exact; the MMA truncates a_lo to 11 bits: 2^-23 |a|)
 //     a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi                       (dropped a_lo.b_lo ~ 2^-24 |a||b|)
 // which keeps fp32-grade accuracy (the parity tolerance is atol 1e-5 / rtol 1e-4; plain TF32 would be ~1e-3).
 //
-// Operand layout (both operands K-major, SWIZZLE_128B, fp32 words): a tile of R rows x 32 k-values is R rows of
-// 128 bytes; 8-row groups are 1024 B apart (SBO); inside a row the 16-byte chunk c sits at position c ^ (row & 7).
-// One tcgen05.mma kind::tf32 consumes K=8 (32 bytes); stepping K inside the swizzled row = advancing the descriptor
-// start address by 32 bytes.
+// Operand layout (both operands K-major, SWIZZLE_128B): a tile of R rows x 128 bytes of k-values; 8-row groups are
+// 1024 B apart (SBO); inside a row the 16-byte chunk c sits at position c ^ (row & 7).  One wgmma consumes 32 bytes of
+// every row (K=8 tf32 or K=16 fp16); stepping K inside the swizzled row = advancing the descriptor start address by 32 bytes.
 #pragma once
 #include <cuda_fp16.h>
 
 #include "dsb_internal.cuh"
+#include "dsb_wgmma.cuh"
 
 namespace dsb {
 namespace tc {
 
-constexpr int TM = 128;            // rows (edges / nodes) per tile = TMEM lanes
+constexpr int TM = 128;            // rows (edges / nodes) per tile: two warpgroups of 64 rows
+constexpr int WG_ROWS = 64;        // rows per warpgroup = M of one wgmma
 constexpr int TKC = 32;            // k-values per 128-byte swizzle row with 4-byte (TF32) operands
 constexpr int TKC16 = 64;          // ... with 2-byte (FP16) operands
 constexpr float X_SCALE = 1.0f;    // 3xFP16 activation scale (1: |x| < 0.25 has a subnormal fp16 residual, abs. error <= 3e-8)
 constexpr int A_CHUNK_BYTES = TM * 128;        // 16 KB
 constexpr int NSTAGE = 2;
-constexpr int ACC_STRIDE = 256;    // TMEM column offset of the second accumulator (512 columns are allocated for every width)
+constexpr int MMA_THREADS = 256;   // two warpgroups: each builds the A operand of its 64 rows, issues its wgmmas and runs the epilogue
+constexpr int TC_THREADS = MMA_THREADS + 128;  // + a third warpgroup whose lane 0 streams the weight chunks (keeps the MMA
+                                               //   warpgroups free of single-thread branches while their wgmmas are in flight)
+// register split (setmaxnreg): the weight warpgroup gives its registers to the two MMA warpgroups, which hold H/2
+// accumulators per thread: 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int WEIGHT_WG_REGS = 40, MMA_WG_REGS = 232;
+template <int R> __device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // Geometry that depends on the width H = hidden_nf of the network (128, 192 or 256): the accumulator tile is TM x H, a weight
 // chunk image is H rows x 128 B.
 template <int H>
 struct Geo {
   static_assert(H == 128 || H == 192 || H == 256, "tensor-core kernels are built for hidden_nf 128, 192, 256");
-  static constexpr int TN = H;                                  // accumulator columns per tile = N of one MMA
+  static constexpr int TN = H;                                  // accumulator columns per tile = N of one wgmma
+  static constexpr int ACC = H / 2;                             // fp32 accumulator registers per thread
   static constexpr int B_CHUNK_BYTES = H * 128;                 // 16 / 24 / 32 KB
   static constexpr int B_CHUNK_FLOATS = H * TKC;                // 32-bit words per chunk image
   static constexpr int STAGE_BYTES = 2 * A_CHUNK_BYTES + 2 * B_CHUNK_BYTES;   // Xhi, Xlo, Whi, Wlo = 64 / 80 / 96 KB
-  // instruction descriptor: D=F32, K-major both, N=H, M=128  (cute::UMMA::InstrDescriptor bit layout); A=B=TF32 (code 2) / F16 (0)
-  static constexpr uint32_t IDESC_TF32 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(H >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-  static constexpr uint32_t IDESC_F16 = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(H >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
 };
-
-constexpr int EPI_WARPS = 4;       // warps 0..3  (warp w owns TMEM lanes 32w..32w+31)
-constexpr int PROD_WARPS = 8;      // warps 4..11
-constexpr int MMA_WARP = EPI_WARPS + PROD_WARPS;        // 12
-constexpr int TMA_WARP = MMA_WARP + 1;                  // 13
-constexpr int TC_THREADS = (TMA_WARP + 1) * 32;         // 448
-constexpr int PROD_THREADS = PROD_WARPS * 32;           // 256
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -59,15 +58,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_n(uint64_t* bar, uint32_t n) {       // one thread arriving for n participants
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(n) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-// try_wait with an explicit suspend-time hint: the thread sleeps in hardware until the phase completes (or ~20 us pass)
-// instead of re-polling every few tens of cycles -- the default time limit made the waiting roles (MMA/TMA issuers, scalar
-// warps) spend ~25 % of the SM's issue slots on SYNCS/BRA/ISETP polling next to the working warps (ncu source view).
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -79,177 +72,70 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded spin: a protocol bug must trap (CUDA error) instead of hanging the GPU.
+// Bounded spin: a protocol bug must trap (CUDA error) instead of hanging the GPU.  The trap is a predicated instruction,
+// not a branch, and there is no printf (a call): either would put a divergent path between a wgmma and its wait, which
+// makes ptxas serialise the wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 17)) { printf("dsb tc: mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+    ++spins;
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.gt.u32 p, %0, %1;\n\t@p trap;\n\t}" ::"r"(spins), "r"(1u << 17));
   }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// barrier over the 128 threads of warpgroup wg (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(wg + 1) : "memory"); }
 
-// ---- bulk copy global -> shared (UBLKCP), completion on an mbarrier -------------------------------------------------
+// ---- bulk copy global -> shared, completion on an mbarrier -------------------------------------------------------------
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// ---- TMEM ----------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {   // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma ---------------------------------------------------------------------------------------------------------
+// K-major SWIZZLE_128B shared-memory descriptor: start>>4 | LBO (unused for this layout, 1) <<16 | SBO (1024>>4) <<32 |
+// layout SWIZZLE_128B (1) <<62.  Tiles start 1024-byte aligned, so the base offset field stays 0.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {         // same warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive columns: thread i of the warp gets lane (base_lane + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  // the registers are only valid after tcgen05.wait::ld; keep the wait fused here so no use can be scheduled before it
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-  uint32_t r[32];
+
+// The 12 wgmmas of one K-chunk held in stage memory `st` (A_hi | A_lo | W_hi | W_lo) for the 64 rows of warpgroup wg:
+// 4 k-steps x 3 split products into d; the first product of a tile's first chunk overwrites d.  first_chunk only sets the
+// scale-d predicate of one instruction: no branch around the wgmmas (a divergent path between a wgmma and its wait makes
+// ptxas serialise the pipeline).
+template <bool F16, int H>
+__device__ __forceinline__ void mma_chunk(float (&d)[H / 2], const char* st, int wg, bool first_chunk) {
+  using G = Geo<H>;
+  const uint32_t xhi = smem_u32(st) + (uint32_t)(wg * WG_ROWS * 128), xlo = xhi + A_CHUNK_BYTES;
+  const uint32_t whi = smem_u32(st) + 2 * A_CHUNK_BYTES, wlo = whi + G::B_CHUNK_BYTES;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(v[i]);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-
-// split form for software pipelining: issue now, consume after tmem_ld32_wait(r).  The wait carries the 32 registers as
-// in/out operands so that no use of them can be scheduled above it.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-      : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-        "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-        "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-        "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-      :: "memory");
-}
-
-// ---- UMMA ----------------------------------------------------------------------------------------------------------
-// K-major SWIZZLE_128B shared-memory descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO(1)<<16 | SBO(1024>>4)<<32 |
-// version 1 <<46 | layout SWIZZLE_128B(2) <<61
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all previously issued MMAs of this thread arrive on the mbarrier when they complete (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- CTA pair (cluster of 2, tcgen05 cta_group::2) ----------------------------------------------------------------------
-// The leader CTA (cluster rank 0) issues tcgen05.mma.cta_group::2 for both: M = 256 = the two CTAs' 128 operand rows each (A
-// descriptor: the same shared-memory offset in both CTAs), B = N/2 rows per CTA at one offset, accumulators in each CTA's own
-// TMEM.  Hand-offs that involve the other CTA are mbarrier arrives on the leader's barriers through the cluster address space
-// (release / acquire at cluster scope) and multicast commits.
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {          // every thread of both CTAs
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// shared::cluster address of the leader CTA's copy of a shared-memory object
-__device__ __forceinline__ uint32_t leader_addr(const void* p) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, 0;" : "=r"(r) : "r"(smem_u32(p)));
-  return r;
-}
-// Default semantics (release at CTA scope), as CUTLASS's ClusterBarrier::arrive: what is handed over lives in the arriving
-// CTA's own shared memory / TMEM (made visible to the async proxy by fence.proxy.async resp. ordered by tcgen05.fence before
-// the arrive) and is consumed by tensor-core hardware, not by another SM's loads.  The .release.cluster form compiles to
-// MEMBAR.ALL.GPU, which would stall every hand-off on the thread's prefetched gathers.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P1;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2, %3;\n\t"
-      "selp.b32 %0, 1, 0, P1;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(20000u)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (++spins > (1u << 17)) { printf("dsb tc: cluster mbarrier timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x); __trap(); }
+  for (int ks = 0; ks < 4; ++ks) {       // 4 k-steps of 32 bytes per 128-byte row (K=8 tf32 or K=16 fp16 each)
+    const uint32_t ko = ks * 32;
+    const uint32_t acc = (first_chunk && ks == 0) ? 0u : 1u;
+    if constexpr (F16) {
+      Wgmma<H>::f16(d, wgmma_desc_sw128(xlo + ko), wgmma_desc_sw128(whi + ko), acc);
+      Wgmma<H>::f16(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(wlo + ko), 1u);
+      Wgmma<H>::f16(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(whi + ko), 1u);
+    } else {
+      Wgmma<H>::tf32(d, wgmma_desc_sw128(xlo + ko), wgmma_desc_sw128(whi + ko), acc);
+      Wgmma<H>::tf32(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(wlo + ko), 1u);
+      Wgmma<H>::tf32(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(whi + ko), 1u);
+    }
   }
 }
-__device__ __forceinline__ void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) {   // one full warp in EACH CTA of the pair
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// all previously issued MMAs of this thread arrive on the barrier at this shared-memory offset in BOTH CTAs when they complete
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
 
-// round-to-nearest (ties away) to the 19-bit TF32 container with two integer-pipe instructions (cvt.rna.tf32.f32
-// would occupy the 16-lane XU pipe that the SiLU exponentials already saturate)
+// round-to-nearest (ties away) to the 19-bit TF32 container with two integer-pipe instructions
 __device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
 
 // byte offset of (row r, 16-byte chunk c) inside a [rows][128 B] SWIZZLE_128B tile
@@ -257,97 +143,32 @@ __device__ __host__ __forceinline__ uint32_t sw128_offset(int r, int c) {
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
 }
 
-// producer helper: split 4 consecutive k-values and store them (hi, lo) at (row, chunk) of the stage's A tiles
-__device__ __forceinline__ void store_split(char* a_hi, char* a_lo, int row, int chunk, float4 v) {
-  float4 h = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
-  float4 l = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
-  const uint32_t off = sw128_offset(row, chunk);
-  *reinterpret_cast<float4*>(a_hi + off) = h;
-  *reinterpret_cast<float4*>(a_lo + off) = l;
-}
-
-// Residual of the 3xFP16 split, x - float(hi), for a packed pair of fp16 hi parts: one mixed-precision FMA per value
-// (fma.rn.f32.f16 = FHFMA: hi * (-1) + x, exact) instead of a half->float conversion plus a subtraction.  Same bits as
-// x - __half2float(hi): the difference is representable in fp32.
+// Residual of the 3xFP16 split, x - float(hi), for a packed pair of fp16 hi parts (exact: the difference is
+// representable in fp32).
 __device__ __forceinline__ void residual_f16(uint32_t hi2, float x0, float x1, float& r0, float& r1) {
-  asm("{.reg .f16 l, h; mov.b32 {l, h}, %2; fma.rn.f32.f16 %0, l, %3, %4; fma.rn.f32.f16 %1, h, %3, %5;}"
-      : "=f"(r0), "=f"(r1) : "r"(hi2), "h"((unsigned short)0xBC00), "f"(x0), "f"(x1));
+  const __half2 h = *reinterpret_cast<const __half2*>(&hi2);
+  r0 = x0 - __low2float(h);
+  r1 = x1 - __high2float(h);
 }
 __device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
-// 3xFP16 producer helper: 8 consecutive k-values (two float4, already multiplied by X_SCALE) -> 16-byte chunk c16 of the
-// row in the hi and lo tiles.  x_h = fp16_rn(x), x_l = fp16_rn(x - x_h): 22 significand bits while x_l is a normal fp16.
-__device__ __forceinline__ void store_split_f16(char* a_hi, char* a_lo, int row, int c16, float4 v0, float4 v1) {
-  const __half2 h0 = __floats2half2_rn(v0.x, v0.y), h1 = __floats2half2_rn(v0.z, v0.w);
-  const __half2 h2 = __floats2half2_rn(v1.x, v1.y), h3 = __floats2half2_rn(v1.z, v1.w);
-  float r0, r1, r2, r3, r4, r5, r6, r7;
-  residual_f16(h2_bits(h0), v0.x, v0.y, r0, r1); residual_f16(h2_bits(h1), v0.z, v0.w, r2, r3);
-  residual_f16(h2_bits(h2), v1.x, v1.y, r4, r5); residual_f16(h2_bits(h3), v1.z, v1.w, r6, r7);
-  const __half2 l0 = __floats2half2_rn(r0, r1), l1 = __floats2half2_rn(r2, r3);
-  const __half2 l2 = __floats2half2_rn(r4, r5), l3 = __floats2half2_rn(r6, r7);
-  const uint32_t off = sw128_offset(row, c16);
-  uint4 hv, lv;
-  hv.x = *reinterpret_cast<const uint32_t*>(&h0); hv.y = *reinterpret_cast<const uint32_t*>(&h1);
-  hv.z = *reinterpret_cast<const uint32_t*>(&h2); hv.w = *reinterpret_cast<const uint32_t*>(&h3);
-  lv.x = *reinterpret_cast<const uint32_t*>(&l0); lv.y = *reinterpret_cast<const uint32_t*>(&l1);
-  lv.z = *reinterpret_cast<const uint32_t*>(&l2); lv.w = *reinterpret_cast<const uint32_t*>(&l3);
-  *reinterpret_cast<uint4*>(a_hi + off) = hv;
-  *reinterpret_cast<uint4*>(a_lo + off) = lv;
-}
 
-// Producer-side store of 4 consecutive k-values (piece p = k/4 of the 32-k half `half`) of one tile row.
-//   TF32: chunk (stage) = one 32-k half: 16-byte stores at chunk position p
-//   FP16: chunk (stage) = two halves (64 k): 8-byte stores at byte (half&1)*64 + 8p of the row
+// Producer-side store of 4 consecutive k-values of one tile row at `dst` (stage base + swizzled offset of the row piece):
+//   TF32: 16-byte stores (hi tile, lo tile A_CHUNK_BYTES further)
+//   FP16: 8-byte stores
 // An FP16 activation beyond the fp16 range becomes inf here and reaches the output as NaN -> the NaN guard of the
-// denoiser raises (dynamics.py:155-159 convention); 3xTF32 has no such limit.
-template <bool F16>
-__device__ __forceinline__ void store_piece(char* st, int row, int half, int p, float4 v) {
-  if constexpr (F16) {
-    const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
-    float r0, r1, r2, r3;
-    residual_f16(h2_bits(h0), v.x, v.y, r0, r1); residual_f16(h2_bits(h1), v.z, v.w, r2, r3);
-    const __half2 l0 = __floats2half2_rn(r0, r1), l1 = __floats2half2_rn(r2, r3);
-    const uint32_t off = sw128_offset(row, (half & 1) * 4 + (p >> 1)) + (p & 1) * 8;
-    uint2 hv, lv;
-    hv.x = *reinterpret_cast<const uint32_t*>(&h0); hv.y = *reinterpret_cast<const uint32_t*>(&h1);
-    lv.x = *reinterpret_cast<const uint32_t*>(&l0); lv.y = *reinterpret_cast<const uint32_t*>(&l1);
-    *reinterpret_cast<uint2*>(st + off) = hv;
-    *reinterpret_cast<uint2*>(st + A_CHUNK_BYTES + off) = lv;
-  } else {
-    store_split(st, st + A_CHUNK_BYTES, row, p, v);
-  }
-}
-
-// Same split as store_piece, for a row piece already held as two packed pairs and a precomputed destination address
-// (stage base + swizzled offset of the row piece): the residual is one packed subtraction.
-__device__ __forceinline__ f32x2 sub2_(f32x2 a, f32x2 b) { f32x2 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-#ifndef DSB_SPLIT_TRUNC
-#define DSB_SPLIT_TRUNC 0
-#endif
+// denoiser raises; 3xTF32 has no such limit.
 template <bool F16>
 __device__ __forceinline__ void store_pair(char* dst, f32x2 u01, f32x2 u23) {
   float x0, x1, x2, x3;
   upk2(u01, x0, x1); upk2(u23, x2, x3);
   if constexpr (F16) {
-#if DSB_SPLIT_TRUNC
-    // hi = x with the 13 low mantissa bits cleared (exactly representable in fp16 when normal there): four LOP3 on the ALU pipe
-    // instead of four half->float conversions on the FMA pipe; the residual is < 2^-10 |x| (rounding: 2^-11), kept to 11 bits
-    const float t0 = __uint_as_float(__float_as_uint(x0) & 0xffffe000u), t1 = __uint_as_float(__float_as_uint(x1) & 0xffffe000u);
-    const float t2 = __uint_as_float(__float_as_uint(x2) & 0xffffe000u), t3 = __uint_as_float(__float_as_uint(x3) & 0xffffe000u);
-    const __half2 h0 = __floats2half2_rn(t0, t1), h1 = __floats2half2_rn(t2, t3);
-    const float2 f0 = make_float2(t0, t1), f1 = make_float2(t2, t3);
-#else
     const __half2 h0 = __floats2half2_rn(x0, x1), h1 = __floats2half2_rn(x2, x3);
-#endif
     float l0, l1, l2, l3;
-#if DSB_SPLIT_TRUNC
-    upk2(sub2_(u01, pk2(f0.x, f0.y)), l0, l1); upk2(sub2_(u23, pk2(f1.x, f1.y)), l2, l3);
-#else
     residual_f16(h2_bits(h0), x0, x1, l0, l1); residual_f16(h2_bits(h1), x2, x3, l2, l3);
-#endif
     const __half2 q0 = __floats2half2_rn(l0, l1), q1 = __floats2half2_rn(l2, l3);
     uint2 hv, lv;
-    hv.x = *reinterpret_cast<const uint32_t*>(&h0); hv.y = *reinterpret_cast<const uint32_t*>(&h1);
-    lv.x = *reinterpret_cast<const uint32_t*>(&q0); lv.y = *reinterpret_cast<const uint32_t*>(&q1);
+    hv.x = h2_bits(h0); hv.y = h2_bits(h1);
+    lv.x = h2_bits(q0); lv.y = h2_bits(q1);
     *reinterpret_cast<uint2*>(dst) = hv;
     *reinterpret_cast<uint2*>(dst + A_CHUNK_BYTES) = lv;
   } else {
@@ -356,105 +177,62 @@ __device__ __forceinline__ void store_pair(char* dst, f32x2 u01, f32x2 u23) {
     *reinterpret_cast<float4*>(dst + A_CHUNK_BYTES) = make_float4(x0 - h.x, x1 - h.y, x2 - h.z, x3 - h.w);
   }
 }
+// byte offset of row r's piece p (4 k-values, p in 0..7) of 32-k half hf inside a stage's A tile
+template <bool F16>
+__device__ __forceinline__ uint32_t piece_offset(int r, int hf, int p) {
+  return F16 ? sw128_offset(r, (hf & 1) * 4 + (p >> 1)) + (uint32_t)(p & 1) * 8u : sw128_offset(r, p);
+}
 
-// ---- shared-memory control block -------------------------------------------------------------------------------------
+// ---- weight pipeline --------------------------------------------------------------------------------------------------
+// Stage s holds one K-chunk: A_hi | A_lo (built by the warpgroups, each its own 64 rows) | W_hi | W_lo (bulk copies).
+// full_w[s]: the weight chunk has landed (1 arrive + tx bytes).  empty[s]: the wgmmas that read the stage have completed
+// in all 8 warps of both warpgroups (one arrive per warp), so the next weight chunk may be copied in.
 struct Control {
-  uint64_t full_x[NSTAGE];     // producers -> MMA   (count PROD_WARPS)
-  uint64_t full_w[NSTAGE];     // TMA -> MMA         (count 1 + tx bytes)
-  uint64_t empty[NSTAGE];      // MMA commit -> producers, TMA (count 1)
-  uint64_t acc_full[2];        // MMA commit -> epilogue (count 1)
-  uint64_t epi_done[2];        // epilogue -> MMA, producers (count EPI_WARPS)
-  uint64_t scal_full[3];       // scalar warps -> producers, epilogue (count SCAL_WARPS): per-edge scalars of the tile are in shared memory
-  uint64_t scal_empty[3];      // epilogue -> scalar warps (count EPI_WARPS): scalar buffers of the tile may be overwritten
-  uint64_t w_full;             // CTA-pair edge kernels: bulk copies of this CTA's resident weight half (count 1 + tx bytes)
-  uint64_t w_ready;            // ... leader only: both CTAs' weight halves are in shared memory (count 2)
-  uint32_t tmem_base;
-  uint32_t pad;
+  uint64_t full_w[NSTAGE];
+  uint64_t empty[NSTAGE];
 };
 
-__device__ __forceinline__ void control_init(Control* c, int scal_full_count) {
-  for (int s = 0; s < NSTAGE; ++s) { mbar_init(&c->full_x[s], PROD_WARPS); mbar_init(&c->full_w[s], 1); mbar_init(&c->empty[s], 1); }
-  for (int a = 0; a < 2; ++a) { mbar_init(&c->acc_full[a], 1); mbar_init(&c->epi_done[a], EPI_WARPS); }
-  for (int a = 0; a < 3; ++a) { mbar_init(&c->scal_full[a], scal_full_count); mbar_init(&c->scal_empty[a], EPI_WARPS); }
+__device__ __forceinline__ void control_init(Control* c) {
+  for (int s = 0; s < NSTAGE; ++s) { mbar_init(&c->full_w[s], 1); mbar_init(&c->empty[s], 8); }
   fence_barrier_init();
 }
 
-// ---- MMA issuer (one thread): per tile, per chunk: 4 k-steps x 3 split products ------------------------------------------
-// bring-up / diagnosis switch (see dsb_tc.cu); this header is included by exactly one translation unit
-__device__ int g_tc_debug = 0;
-// Product build: the switch is a compile-time 0, so every ablation branch and cycle counter below folds away.  The
-// instrumented library (libdiffsbdd_b200_instr.so, -DDSB_TC_INSTRUMENT=1, selected with DSB_INSTRUMENT=1) reads it at run time.
-#ifndef DSB_TC_INSTRUMENT
-#define DSB_TC_INSTRUMENT 0
-#endif
-__device__ __forceinline__ int tc_debug() {
-#if DSB_TC_INSTRUMENT
-  return g_tc_debug;
-#else
-  return 0;
-#endif
-}
-// cycle accounting of one epilogue warp and one producer warp per CTA (enabled by g_tc_debug & 512; profiles/tc_ablate.py)
-__device__ unsigned long long g_tc_prof[64];
-__device__ __forceinline__ long long tc_clock() { return clock64(); }
-// the 12 MMAs of one K-chunk held in stage memory `st` (A_hi | A_lo | W_hi | W_lo): 4 k-steps x 3 split products into d
-template <bool F16, int H>
-__device__ __forceinline__ void mma_issue_chunk(uint32_t d, char* st, bool first_chunk) {
-  using G = Geo<H>;
-  const uint32_t xhi = smem_u32(st), xlo = xhi + A_CHUNK_BYTES, whi = xhi + 2 * A_CHUNK_BYTES, wlo = whi + G::B_CHUNK_BYTES;
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {       // 4 k-steps of 32 bytes per 128-byte row (K=8 tf32 or K=16 fp16 each)
-    const uint32_t ko = ks * 32;
-    const uint32_t acc = (first_chunk && ks == 0) ? 0u : 1u;
-    if constexpr (F16) {
-      umma_f16(d, umma_desc_sw128(xlo + ko), umma_desc_sw128(whi + ko), G::IDESC_F16, acc);
-      umma_f16(d, umma_desc_sw128(xhi + ko), umma_desc_sw128(wlo + ko), G::IDESC_F16, 1u);
-      umma_f16(d, umma_desc_sw128(xhi + ko), umma_desc_sw128(whi + ko), G::IDESC_F16, 1u);
-    } else {
-      umma_tf32(d, umma_desc_sw128(xlo + ko), umma_desc_sw128(whi + ko), G::IDESC_TF32, acc);
-      umma_tf32(d, umma_desc_sw128(xhi + ko), umma_desc_sw128(wlo + ko), G::IDESC_TF32, 1u);
-      umma_tf32(d, umma_desc_sw128(xhi + ko), umma_desc_sw128(whi + ko), G::IDESC_TF32, 1u);
-    }
+// Sequence of K-chunks g = 0, 1, ... of a CTA (all tiles in order), issued by lane 0 of the weight warp: chunk g goes into
+// stage g % 2 once chunk g - 2 (same stage) has been consumed by both warpgroups.
+template <int H>
+struct WeightStream {
+  Control* ctl;
+  char* stages;
+  __device__ void issue(uint32_t g, const float* hi, const float* lo) const {
+    using G = Geo<H>;
+    const int s = g & 1;
+    if (g >= NSTAGE) mbar_wait(&ctl->empty[s], ((g >> 1) - 1) & 1);
+    char* st = stages + (size_t)s * G::STAGE_BYTES + 2 * A_CHUNK_BYTES;
+    mbar_arrive_expect_tx(&ctl->full_w[s], 2 * G::B_CHUNK_BYTES);
+    bulk_g2s(st, hi, G::B_CHUNK_BYTES, &ctl->full_w[s]);
+    bulk_g2s(st + G::B_CHUNK_BYTES, lo, G::B_CHUNK_BYTES, &ctl->full_w[s]);
   }
-}
+};
 
-template <bool F16, int H>
-__device__ __forceinline__ void mma_role(Control* ctl, char* stages, int n_my_tiles, int chunks_per_tile, int tag) {
-  const uint32_t tmem = ctl->tmem_base;
-  const bool skip = (tc_debug() & 8) != 0;
-  // cycle accounting of the issuing thread (g_tc_debug & 512): slots 32 + 8 tag + {0: wait accumulator, 1: wait W, 2: wait X,
-  // 3: issue, 4: chunks}; tag 0 = node GEMM, 1 = GCL, 2 = coord
-  const bool mprof = (tc_debug() & 512) != 0;
-  long long w_acc = 0, w_w = 0, w_x = 0, w_iss = 0, q0 = 0, q1 = 0, q2 = 0, q3 = 0;
-  uint32_t g = 0;
-  for (int it = 0; it < n_my_tiles; ++it) {
-    const int a = it & 1;
-    if (mprof) q0 = tc_clock();
-    mbar_wait(&ctl->epi_done[a], ((it >> 1) & 1) ^ 1);      // accumulator buffer drained by the epilogue
-    tc_fence_after();
-    if (mprof) w_acc += tc_clock() - q0;
-    const uint32_t d = tmem + (uint32_t)(a * ACC_STRIDE);
-    for (int kc = 0; kc < chunks_per_tile; ++kc, ++g) {
-      const int s = g & 1;
-      const uint32_t par = (g >> 1) & 1;
-      if (mprof) q0 = tc_clock();
-      mbar_wait(&ctl->full_w[s], par);
-      if (mprof) q1 = tc_clock();
-      mbar_wait(&ctl->full_x[s], par);
-      tc_fence_after();
-      if (mprof) { q2 = tc_clock(); w_w += q1 - q0; w_x += q2 - q1; }
-      if (!skip) mma_issue_chunk<F16, H>(d, stages + (size_t)s * Geo<H>::STAGE_BYTES, kc == 0);
-      umma_commit(&ctl->empty[s]);          // stage reusable once these MMAs have read it
-      if (mprof) { q3 = tc_clock(); w_iss += q3 - q2; }
+// Per-warpgroup bookkeeping of the asynchronous wgmma groups: every chunk's stage is released (one arrive on empty) once
+// its wgmmas are known to be complete (lane 0 of every warp arrives).  At most one group stays in flight while the next
+// chunk's operand is built.
+struct MmaTracker {
+  int pend = -1;
+  template <int H>
+  __device__ __forceinline__ void after_commit(Control* ctl, float (&d)[H / 2], int g, bool last_of_tile, bool leader) {
+    if (last_of_tile) {
+      wgmma_wait<0>();
+      acc_fence(d);
+      if (leader) { if (pend >= 0) mbar_arrive(&ctl->empty[pend & 1]); mbar_arrive(&ctl->empty[g & 1]); }
+      pend = -1;
+    } else {
+      wgmma_wait<1>();
+      if (leader && pend >= 0) mbar_arrive(&ctl->empty[pend & 1]);
+      pend = g;
     }
-    umma_commit(&ctl->acc_full[a]);         // accumulator complete
   }
-  if (mprof) {
-    unsigned long long* o = g_tc_prof + 32 + 8 * tag;
-    atomicAdd(o + 0, (unsigned long long)w_acc); atomicAdd(o + 1, (unsigned long long)w_w); atomicAdd(o + 2, (unsigned long long)w_x);
-    atomicAdd(o + 3, (unsigned long long)w_iss); atomicAdd(o + 4, (unsigned long long)n_my_tiles * chunks_per_tile);
-  }
-}
+};
 
 }  // namespace tc
 }  // namespace dsb

@@ -1,4 +1,4 @@
-"""Drop-in ``EGNNDynamics`` whose forward runs on the hand-written sm_100a kernels.
+"""Drop-in ``EGNNDynamics`` whose forward runs on the hand-written sm_90a kernels.
 
 Mirrors the reference module (equivariant_diffusion/dynamics.py:10-187): same constructor signature,
 same attribute names callers read (``update_pocket_coords``, ``n_dims``, ``edge_cutoff_{l,p,i}``,
@@ -149,7 +149,7 @@ class EGNNDynamics(nn.Module):
         self._workspace: Optional[torch.Tensor] = None
         self._status: Optional[torch.Tensor] = None
         self.defer_status_check = False    # samplers that CUDA-graph the loop check once at the end
-        # arithmetic path: bitmask 1 node GEMMs | 2 edge kernel | 4 coordinate kernel on tcgen05, 8 = 3xFP16 operand split
+        # arithmetic path: bitmask 1 node GEMMs | 2 edge kernel | 4 coordinate kernel on wgmma, 8 = 3xFP16 operand split
         # instead of 3xTF32; 0 = fp32 FFMA kernels.  Names: 'fp32' (0), '3xtf32' (7), '3xfp16' (15).
         # 'auto' = '3xfp16' when hidden_nf is 128, 192 or 256 (the widths with tensor-core kernels), else 'fp32'.
         self._math_mode = os.environ.get('DSB_MATH_MODE', 'auto')
@@ -247,8 +247,7 @@ class EGNNDynamics(nn.Module):
         ws = self._workspace.data_ptr() if self._workspace is not None else 0
         stt = self._status.data_ptr() if self._status is not None else 0
         pdl = int(_native.load().dsb_set_programmatic_launch(-1))
-        kv = int(_native.load().dsb_set_kernel_variants(-1))
-        return (self._handle_gen, self._handle, self.math_mode, ws, stt, pdl, kv)
+        return (self._handle_gen, self._handle, self.math_mode, ws, stt, pdl)
 
     def _scratch(self, device, n_atoms, n_res, n_graphs, ecap) -> torch.Tensor:
         lib = _native.load()

@@ -1,5 +1,5 @@
 /*
- * diffsbdd_b200 — C ABI of the B200-native DiffSBDD denoiser hot path.
+ * diffsbdd_b200 — C ABI of the H100-native (sm_90a) DiffSBDD denoiser hot path.
  *
  * The reference has no FFI: its "plugin point" is the Python call
  *     EGNNDynamics.forward(xh_atoms, xh_residues, t, mask_atoms, mask_residues)
@@ -131,22 +131,13 @@ int dsb_dynamics_last_launch_count(const dsb_dynamics* dyn);
  * environment variable DSB_PDL (default on).  No effect on results. */
 int dsb_set_programmatic_launch(int enable);
 
-/* Process-wide selection among equivalent kernel forms of the 3xFP16 path (same results within the parity tolerance).
- * Bit 0: the edge kernels run as CTA pairs (tcgen05 cta_group::2) with the second-layer weights resident in shared memory
- * instead of single CTAs that stream them; bit 1: node_model and the merged first-layer GEMM of a block run as one fused
- * CTA-pair kernel instead of two launches; bit 2: that kernel stops after the node update and the merged GEMM runs as a
- * separate, evenly loaded CTA-pair GEMM fed by bulk copies of an operand image of h.  variants < 0 = query only.  Returns
- * the previous setting.  Initial value: 3 (bit 2 measured equal to the fused form, one launch more), minus bit 0 / 1 if the
- * environment has DSB_EDGE_PAIR=0 / DSB_NODE_BLOCK=0, plus bit 2 if DSB_NODE_SPLIT=1. */
-int dsb_set_kernel_variants(int variants);
-
 /* ---- arithmetic path.  mode is a bitmask: 1 = node GEMMs, 2 = edge (GCL) kernel, 4 = coordinate edge kernel run on
- * the tensor pipe (tcgen05.mma, accumulators in TMEM) as 3-product split contractions with fp32 accumulation
+ * the tensor pipe (wgmma, accumulators in registers) as 3-product split contractions with fp32 accumulation
  * (x.w ~= x_lo.w_hi + x_hi.w_lo + x_hi.w_hi: fp32-grade accuracy, inside the atol 1e-5 / rtol 1e-4 parity tolerance);
- * 8 selects the operand format of those kernels: 0 = 3xTF32 (kind::tf32, 8-bit exponent, any range),
- * 8 = 3xFP16 (kind::f16: half the shared-memory operand traffic, twice the MMA rate; weights are pre-scaled per matrix
+ * 8 selects the operand format of those kernels: 0 = 3xTF32 (tf32 operands, 8-bit exponent, any range),
+ * 8 = 3xFP16 (f16 operands: half the shared-memory operand traffic, twice the MMA rate; weights are pre-scaled per matrix
  * with an exact power of two; an activation beyond the fp16 range turns into NaN at the output and raises through
- * status[0]).  0 = fp32 FFMA kernels everywhere.  Only hidden_nf == 256 has tensor-core kernels. */
+ * status[0]).  0 = fp32 FFMA kernels everywhere.  Only hidden_nf 128, 192 and 256 have tensor-core kernels. */
 int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode);
 
 /* ---- measurement hook (bench.py's live roofline).  When enabled, every non-captured forward brackets
@@ -213,14 +204,6 @@ int dsb_ddpm_joint_inpaint_update(float* z_lig, float* z_pocket, const float* xh
 
 const char* dsb_last_error(void);
 const char* dsb_version(void);
-
-/* ---- diagnostics of the tensor-core kernels (profiles/tc_ablate.py; no reference counterpart).  The product library is
- * built without instrumentation: dsb_debug_set_tc_flags(flags != 0) returns -4 and the counters stay 0.  The instrumented
- * build (-DDSB_TC_INSTRUMENT=1, libdiffsbdd_b200_instr.so) takes a bitmask that disables individual roles of the kernels
- * (results are then garbage) and, with bit 512, accumulates in-kernel clock64 counters that dsb_debug_read_tc_prof copies
- * into out64[64] and clears. */
-int dsb_debug_set_tc_flags(int flags);
-int dsb_debug_read_tc_prof(unsigned long long* out64);
 
 #ifdef __cplusplus
 }

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — nn.Module wrapper giving the oracle the ``EGNNDynamics`` call contract
 (reference dynamics.py:87), so the DDPM samplers can be driven on CPU: used by the wrapper parity tests
-and by bench.py's CPU-baseline / ``--impl reference`` legs (kind "port": the reference itself cannot
-travel to the GPU box)."""
+and by bench.py's CPU-baseline / ``--impl reference`` legs (kind "port": the benchmark does not need the
+reference checkout)."""
 import torch.nn as nn
 
 from . import egnn_oracle

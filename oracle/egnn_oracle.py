@@ -3,13 +3,12 @@
 A functional, state-dict-driven restatement of what ``EGNNDynamics.forward`` computes in the
 reference (dynamics.py:87-167 -> egnn_new.py:225-244 -> :163-184 -> :60-66, :124-132). It exists so
 that the parity tests, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline leg have a checker
-that travels to the GPU box (where /root/reference does not exist). The product path
+that travels with the repository (the reference checkout is not needed to run them). The product path
 (``diffsbdd_b200``) never imports this module.
 
 Parity pinning: the reference ships no golden vectors (SURVEY.md §8(c)); this oracle is pinned
-instead against outputs of the unmodified reference run in the build container
-(``tests/golden/*.npz`` produced by ``tests/golden/make_golden.py`` through ``oracle/ref_shim.py``),
-and — when /root/reference is present — directly in ``tests/test_oracle_vs_reference.py``.
+instead against stored outputs of the unmodified reference
+(``tests/golden/*.npz`` produced by ``tests/golden/make_golden.py`` through ``oracle/ref_shim.py``).
 
 The op sequence deliberately follows the reference (materialised ``[h_i | h_j | e_ij]`` concatenation,
 whole-batch ``cdist`` adjacency) so that (i) fp32 results agree with the reference to the last bit
@@ -168,7 +167,7 @@ def denoiser_forward(cfg, state_dict: Dict[str, torch.Tensor], xh_atoms, xh_resi
     Returns ``(out_atoms [N_L,3+A], out_residues [N_P,3+R])`` on ``device`` (default CPU: the checker) in ``dtype``;
     raises ``ValueError('NaN detected in EGNN output')`` like dynamics.py:155-159.  ``device='cuda'`` runs the very same
     ATen op sequence on the GPU: that is bench.py's ``--impl reference-gpu`` arm ("the reference's own PyTorch graph on
-    the B200", SURVEY.md §8(d)), never a checker and never the product path."""
+    the GPU", SURVEY.md §8(d)), never a checker and never the product path."""
     if cfg.mode != 'egnn_dynamics':
         raise NotImplementedError('oracle covers mode=egnn_dynamics')
     sd = {k: v.detach().to(device, dtype) for k, v in state_dict.items()}

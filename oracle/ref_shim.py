@@ -1,8 +1,8 @@
-"""TEST INFRASTRUCTURE ONLY — imports the *unmodified* reference from /root/reference.
+"""TEST INFRASTRUCTURE ONLY — imports the *unmodified* reference from the checkout named by the environment
+variable DIFFSBDD_REFERENCE.
 
-Only usable in the build container (the GPU box has no /root/reference). Used by
-``tests/golden/make_golden.py`` to generate the committed golden vectors and by the CPU tests
-that pin ``oracle/egnn_oracle.py`` against the real reference when it is present.
+Used by the generators under ``tests/golden/`` to produce the committed golden data; the tests themselves only
+read that data and never need the reference.
 
 The reference's DDPM wrapper imports ``torch_scatter`` and its top-level ``utils`` imports
 ``rdkit``/``Bio``/``networkx`` at module level (reference utils.py:6-9, en_diffusion.py:8); none is
@@ -20,11 +20,11 @@ import types
 
 import torch
 
-REFERENCE_ROOT = os.environ.get('DIFFSBDD_REFERENCE', '/root/reference')
+REFERENCE_ROOT = os.environ.get('DIFFSBDD_REFERENCE', '')
 
 
 def reference_available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, 'equivariant_diffusion', 'egnn_new.py'))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, 'equivariant_diffusion', 'egnn_new.py'))
 
 
 def _scatter_add(src, index, dim=0, out=None, dim_size=None):
@@ -63,7 +63,7 @@ def _install_stubs():
 def load_reference():
     """Returns a namespace with the reference's own classes (EGNNDynamics, ConditionalDDPM, ...)."""
     if not reference_available():
-        raise RuntimeError(f'reference not found under {REFERENCE_ROOT}')
+        raise RuntimeError(f'reference not found (DIFFSBDD_REFERENCE={REFERENCE_ROOT!r})')
     _install_stubs()
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)

@@ -1,7 +1,7 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (/root/reference, via
-oracle/ref_shim.py) on seeded synthetic inputs and weights. Build-container only.
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (a checkout named by DIFFSBDD_REFERENCE, via
+oracle/ref_shim.py) on seeded synthetic inputs and weights.
 
-    python tests/golden/make_golden.py
+    DIFFSBDD_REFERENCE=<reference checkout> python tests/golden/make_golden.py
 
 Each fixture stores the forward arguments, the reference outputs of ``EGNNDynamics.forward``
 (dynamics.py:87-167), the edge list the reference built (dynamics.py:169-187), the config, the weight
@@ -52,7 +52,7 @@ CASES = {
     'noatt_notanh_l2': (DynamicsConfig(n_layers=2, attention=False, tanh=False, edge_cutoff_ligand=3.0,
                                        hidden_nf=128, joint_nf=32),
                         [20, 15], [40, 50], 9, 4, 0.045, None, (1.0, 4.0)),
-    # ---- hidden_nf=256 variants: the same branches on the tcgen05 kernels (VERDICT r1 "what's weak" #1) ----
+    # ---- hidden_nf=256 variants: the same branches on the tensor-core kernels ----
     # crossdock_ca_joint.yml dims: joint model (all coordinates move, velocity mean removed), residue_nf=20, H=256
     'joint_ca_h256_l6': (DynamicsConfig(update_pocket_coords=True, residue_nf=20), [20, 14, 1], [45, 38, 27], 21, 5,
                          0.007, None, (1.0, 1.0)),

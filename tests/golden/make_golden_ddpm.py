@@ -2,7 +2,7 @@
 (conditional_model.py:479, :558, :364) driven by a CPU denoiser stand-in (the oracle restatement of
 EGNNDynamics.forward, bit-identical to the reference module on CPU — tests/test_oracle_golden.py), with
 fixed torch seeds.  They pin the DDPM wrapper of this repo (schedule, mu/sigma update, COM handling,
-RePaint loop) independently of the CUDA kernels.  Build-container only."""
+RePaint loop) independently of the CUDA kernels.  Needs the reference checkout named by DIFFSBDD_REFERENCE."""
 from __future__ import annotations
 
 import copy

@@ -6,13 +6,30 @@ import os
 import numpy as np
 import torch
 
-from diffsbdd_b200.config import DynamicsConfig
+from diffsbdd_b200.config import CONFIG1, DynamicsConfig
 from diffsbdd_b200 import synthetic as syn
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 # stated fp32 parity tolerance for one denoiser forward (SURVEY.md §4: ~20x the reference's own
 # fp32-vs-fp64 noise floor of 3-4e-7, far below TF32's ~1e-3)
 ATOL, RTOL = 1e-5, 1e-4
+
+# configurations whose reference state-dict layout (keys in order, shapes) is stored in golden/layout/reference_state_dict_layout.npz
+# (golden/make_layout_golden.py): one string array per configuration, entries "<key>:<d0>x<d1>..."
+LAYOUT_CASES = {
+    'config1': CONFIG1,
+    'update_pocket_reflect_h128': DynamicsConfig(update_pocket_coords=True, reflection_equivariant=True, hidden_nf=128),
+    'emb8_h192_l2_noatt': DynamicsConfig(edge_embedding_dim=8, hidden_nf=192, n_layers=2, attention=False),
+}
+
+
+def reference_state_dict_layout(name):
+    entries = np.load(os.path.join(GOLDEN, 'layout', 'reference_state_dict_layout.npz'), allow_pickle=False)[name]
+    out = []
+    for e in entries.tolist():
+        k, shape = e.rsplit(':', 1)
+        out.append((k, tuple(int(d) for d in shape.split('x')) if shape else ()))
+    return out
 
 
 def golden_cases():

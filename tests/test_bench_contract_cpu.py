@@ -1,6 +1,6 @@
 """CPU: the reference arm of bench.py (`--impl reference`, the CPU port of the reference's op sequence on a bounded
 sample) prints ONE JSON line with the contract's keys, on a tiny shape so that it runs in seconds.  The b200 arm needs
-a GPU and is exercised by the driver / `-m gpu` runs; here only its refusal to run without one is checked."""
+a GPU and is exercised on a GPU host; here only its refusal to run without one is checked."""
 import json
 import os
 import subprocess

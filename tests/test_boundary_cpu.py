@@ -10,20 +10,25 @@ from diffsbdd_b200.conditional_model import ConditionalDDPM
 from diffsbdd_b200.dynamics import EGNNDynamics
 from diffsbdd_b200.en_diffusion import EnVariationalDiffusion, DistributionNodes
 from diffsbdd_b200.lightning_modules import LigandPocketDDPM
-from oracle import ref_shim
+from helpers import LAYOUT_CASES, reference_state_dict_layout
 
 
-@pytest.mark.skipif(not ref_shim.reference_available(), reason='/root/reference not mounted')
-@pytest.mark.parametrize('cfg', [CONFIG1, DynamicsConfig(update_pocket_coords=True, reflection_equivariant=True, hidden_nf=128),
-                                 DynamicsConfig(edge_embedding_dim=8, hidden_nf=192, n_layers=2, attention=False)])
+@pytest.mark.parametrize('cfg', list(LAYOUT_CASES.values()))
 def test_state_dict_is_interchangeable_with_reference_module(cfg):
-    ref = ref_shim.load_reference().EGNNDynamics(device='cpu', act_fn=torch.nn.SiLU(), **cfg.kwargs())
+    """The state dict has exactly the reference module's keys, in order, and shapes (stored from the unmodified reference
+    by tests/golden/make_layout_golden.py), so a reference checkpoint loads strictly and this module's state dict loads back."""
+    name = next(n for n, c in LAYOUT_CASES.items() if c is cfg)
+    want = reference_state_dict_layout(name)
     mine = EGNNDynamics.from_config(cfg)
-    r, m = ref.state_dict(), mine.state_dict()
-    assert list(r) == list(m)
-    assert all(r[k].shape == m[k].shape for k in r)
+    m = mine.state_dict()
+    assert [(k, tuple(v.shape)) for k, v in m.items()] == want
+    g = torch.Generator().manual_seed(0)
+    r = {k: torch.randn(shape, generator=g) for k, shape in want}     # a reference checkpoint of that layout
+    if not cfg.reflection_equivariant:                                 # the reference stores the shared last layer twice
+        r = {k: (r[k.replace('cross_product_mlp', 'coord_mlp')] if k.endswith('cross_product_mlp.4.weight') else v)
+             for k, v in r.items()}
     mine.load_state_dict(r, strict=True)                # reference checkpoint -> this module
-    ref.load_state_dict(mine.state_dict(), strict=True)  # and back
+    assert all(torch.equal(mine.state_dict()[k], r[k]) for k in r)
     if not cfg.reflection_equivariant:                  # shared last layer stays shared (egnn_new.py:78)
         q = mine.egnn.e_block_0.gcl_equiv
         assert q.coord_mlp._modules['4'].weight is q.cross_product_mlp._modules['4'].weight
@@ -87,7 +92,7 @@ def test_lightning_facade_builds_and_roundtrips_checkpoint(tmp_path):
     torch.save({'state_dict': model.state_dict(), 'hyper_parameters': _hparams()}, ckpt)
     again = LigandPocketDDPM.load_from_checkpoint(str(ckpt), map_location='cpu')
     for k, v in model.state_dict().items():
-        assert torch.equal(v, again.state_dict()[k])
+        assert torch.equal(v.cpu(), again.state_dict()[k])      # the model itself sits on cuda when a GPU is present
     ca = LigandPocketDDPM(**_hparams(rep='CA'))
     assert ca.aa_nf == 20 and ca.pocket_type_encoder['A'] == 0
     joint = LigandPocketDDPM(**_hparams(mode='joint'))

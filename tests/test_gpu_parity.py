@@ -1,4 +1,4 @@
-"""GPU parity tests proper: the sm_100a kernels, called through the C ABI (libdiffsbdd_b200.so via
+"""GPU parity tests proper: the sm_90a kernels, called through the C ABI (libdiffsbdd_b200.so via
 diffsbdd_b200.EGNNDynamics), against (i) the committed golden vectors produced by the unmodified
 reference and (ii) the travelling CPU oracle on fresh seeded inputs.  Tolerance: atol 1e-5 / rtol 1e-4
 (fp32; helpers.ATOL/RTOL)."""
@@ -39,7 +39,7 @@ def test_golden_edges_bit_exact(case):
 @pytest.mark.parametrize('mode', ['fp32', '3xtf32', 1, 2, 4, 9, 10, 12])
 @pytest.mark.parametrize('case', ['config1_n64_l4', 'ragged_b3_l4', 'fullatom_b2_n200_l6', 'ca_b3_l6'])
 def test_golden_forward_every_math_mode(case, mode):
-    """hidden_nf=256 cases through each arithmetic path: fp32 FFMA kernels; tcgen05 3xTF32 everywhere; and the node
+    """hidden_nf=256 cases through each arithmetic path: fp32 FFMA kernels; wgmma 3xTF32 everywhere; and the node
     GEMMs (1), edge kernel (2), coordinate kernel (4) individually in 3xTF32 and in 3xFP16 (+8).  The default 'auto'
     (= '3xfp16', all kernels) is covered by test_golden_forward."""
     cfg, sd, inp, want, edges = load_golden(case)
@@ -57,7 +57,7 @@ H256_VARIANTS = ['joint_ca_h256_l6', 'reflect_h256_l3', 'sub2_h256_l2', 'noatt_n
 @pytest.mark.parametrize('mode', ['fp32', '3xtf32', '3xfp16'])
 @pytest.mark.parametrize('case', H256_VARIANTS)
 def test_golden_h256_variants_every_arithmetic(case, mode):
-    """The branches the production config does not take, at hidden_nf=256 so that they run on the tcgen05 kernels too:
+    """The branches the production config does not take, at hidden_nf=256 so that they run on the tensor-core kernels too:
     joint mode (all coordinate rows live, velocity mean removal; crossdock_ca_joint.yml dims), reflection-equivariant
     (one coordinate MLP per tile), two sub-layers, no attention / no tanh, the edge-type table of the producers, a
     combination of them, and aggregation_method='mean'.  Goldens come from the unmodified reference (tests/golden/make_golden.py)."""
@@ -76,7 +76,7 @@ OTHER_WIDTHS = ['joint_b2_h128_l5', 'moad_emb8_h192_l3', 'reflect_sub2_nocut_l2'
 @pytest.mark.parametrize('mode', ['fp32', '3xtf32', '3xfp16'])
 @pytest.mark.parametrize('case', OTHER_WIDTHS)
 def test_golden_other_widths_every_arithmetic(case, mode):
-    """hidden_nf 128 and 192 (crossdock_fullatom_joint / moad_* dims, configs/moad_fullatom_cond.yml:32-38): the tcgen05
+    """hidden_nf 128 and 192 (crossdock_fullatom_joint / moad_* dims, configs/moad_fullatom_cond.yml:32-38): the tensor-core
     kernels are templated on the width (accumulator N = H, H/64 pipeline chunks); the fp32 FFMA kernels stay available."""
     cfg, sd, inp, want, edges = load_golden(case)
     net = make_net(cfg, sd)
@@ -137,7 +137,7 @@ def test_forward_does_not_mutate_inputs_and_is_repeatable():
         a2, r2 = net(*dev)
     for x, k in zip(dev, keep):
         assert torch.equal(x, k)
-    # tensor-core path: a receiver's messages are reduced per 32-row warp group and combined with RED.ADD, so the
+    # tensor-core path: a receiver's messages are reduced per 4-row chunk and combined with RED.ADD, so the
     # summation order of >2 partials can vary run to run (fp32 rounding level, like the reference's own scatter_add_ on GPU)
     assert torch.allclose(a1, a2, atol=2e-6, rtol=1e-5) and torch.allclose(r1, r2, atol=2e-6, rtol=1e-5)
     net.math_mode = 'fp32'
@@ -295,35 +295,10 @@ def test_full_batch_oracle_config3():
         print(f'configs[2] full batch, {mode}: E={net.last_num_edges} max abs err ligand {ea:.2e} pocket {er:.2e}')
 
 
-def test_single_cta_kernel_forms_still_match():
-    """dsb_set_kernel_variants(0): the single-CTA edge kernels that stream the weight images and the separate node MLP +
-    merged GEMM launches (the forms 3xTF32 always uses) in 3xFP16, against the golden vectors; then back to the default
-    CTA-pair forms, which must agree with them to rounding."""
-    from diffsbdd_b200 import _native
-    lib = _native.load()
-    cfg, sd, inp, want, edges = load_golden('fullatom_b2_n200_l6')
-    net = make_net(cfg, sd)
-    net.math_mode = '3xfp16'
-    old = lib.dsb_set_kernel_variants(0)
-    try:
-        a = run(net, inp)
-        assert_close(a[0], want[0], 'single-CTA forms, ligand out')
-        assert_close(a[1], want[1], 'single-CTA forms, pocket out')
-        for v in (1, 2, 6, 7):
-            lib.dsb_set_kernel_variants(v)
-            b = run(net, inp)
-            assert_close(b[0], want[0], f'kernel variants {v}, ligand out')
-    finally:
-        lib.dsb_set_kernel_variants(old)
-    assert old == 3
-    c = run(net, inp)
-    assert_close(c[0], a[0], 'pair vs single-CTA forms', atol=3e-6, rtol=1e-5)
-
-
 def test_more_row_tiles_than_cta_pairs():
-    """100 graphs x (25 + 175) nodes = 157 row tiles = 79 tile pairs on 74 CTA pairs: five pairs of the fused node block
-    kernel work on a SECOND item (slot hand-over between items, accumulator phase carried across items).  The graphs whose
-    pocket rows fall into those items must come out as when run alone; one of them is checked against the oracle."""
+    """100 graphs x (25 + 175) nodes = 157 row tiles of the node GEMMs on 132 persistent CTAs: 25 CTAs work on a SECOND
+    tile (weight ring and accumulator carried across tiles).  The graphs whose rows fall into those tiles must come out as
+    when run alone; one of them is checked against the oracle."""
     cfg = FULLATOM_COND
     sd = syn.synthetic_state_dict(cfg, 0)
     B = 100

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, exports every symbol include/diffsbdd_b200.h declares, and its
+"""CPU: the C-ABI library builds for sm_90a, loads, exports every symbol include/diffsbdd_b200.h declares, and its
 host-side logic (parameter table, config validation, size helpers) behaves — no compute calls (no GPU here)."""
 import ctypes as C
 import os
@@ -33,10 +33,10 @@ def test_header_symbols_all_exported(lib):
     assert sorted(_native.EXPORTED_SYMBOLS) == syms
 
 
-def test_library_is_sm100a_only(lib):
+def test_library_is_sm90a_only(lib):
     out = os.popen(f'cuobjdump -lelf {_native.lib_path()} 2>/dev/null').read()
     if out.strip():
-        assert 'sm_100a' in out and not re.search(r'sm_(?!100a)\d+', out), out
+        assert 'sm_90a' in out and not re.search(r'sm_(?!90a)\d+', out), out
 
 
 @pytest.mark.parametrize('cfg', [FULLATOM_COND, CA_COND,
