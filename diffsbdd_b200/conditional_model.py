@@ -3,7 +3,8 @@
 reference: equivariant_diffusion/conditional_model.py — ``sample_given_pocket`` (:479-555), ``inpaint``
 (:558-686), ``diversify`` (:364-409), ``sample_p_zs_given_zt`` (:432-464), ``sample_p_xh_given_z0`` (:112-135),
 ``sample_normal_zero_com`` (:140-160), ``noised_representation`` (:162-183), ``sample_p_zt_given_zs``
-(:420-430), ``remove_mean_batch`` (:688-696), ``SimpleConditionalDDPM`` (:702-746).
+(:420-430), ``remove_mean_batch`` (:688-696), ``SimpleConditionalDDPM`` (:702-746), and the eval-mode likelihood ``forward``
+(:202-330, :727-735) with ``kl_prior``, ``log_pxh_given_z0_without_constants`` and ``log_pN`` (training is not built).
 
 Two loop engines produce the same distribution:
 
@@ -402,6 +403,105 @@ class ConditionalDDPM(EnVariationalDiffusion):
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lmask, pmask
 
+    # ---- evaluation-mode variational bound (conditional_model.py:20-110, :185-330) ---------------------------------------
+    def log_pN(self, N_lig, N_pocket):
+        """log p(N_lig | N_pocket): the ligand size prior given the pocket."""
+        return self.size_distribution.log_prob_n1_given_n2(N_lig, N_pocket)
+
+    def kl_prior(self, xh_lig, mask_lig, num_nodes):
+        """conditional_model.py:20-56: KL of q(z_T | x, h) of the ligand against the standard normal prior."""
+        nd = self.n_dims
+        alpha_T = self.alpha(self.gamma(torch.ones((len(num_nodes), 1), device=xh_lig.device)), xh_lig)
+        mu = alpha_T[mask_lig] * xh_lig
+        return self._kl_prior_from_norms(self.sum_except_batch(mu[:, :nd] ** 2, mask_lig),
+                                         self.sum_except_batch(mu[:, nd:] ** 2, mask_lig), num_nodes, xh_lig.device)
+
+    def _virtual_rows(self, ligand):
+        return ligand['one_hot'][:, self.vnode_idx].bool()
+
+    def log_pxh_given_z0_without_constants(self, ligand, z_0_lig, eps_lig, net_out_lig, gamma_0, epsilon=1e-10):
+        """conditional_model.py:58-110: -1/2 |eps_0.x - net_0.x|^2 (virtual atoms excluded) and log p(h | z_0), ligand only."""
+        nd = self.n_dims
+        sigma_0_cat = self.sigma(gamma_0, target_tensor=z_0_lig) * self.norm_values[1]
+        sq = (eps_lig[:, :nd] - net_out_lig[:, :nd]) ** 2
+        if self.vnode_idx is not None:
+            sq[self._virtual_rows(ligand)] = 0
+        log_px = -0.5 * self.sum_except_batch(sq, ligand['mask'])
+        return log_px, self._log_ph_given_z0(ligand['one_hot'], z_0_lig[:, nd:], sigma_0_cat, ligand['mask'], epsilon)
+
+    def _native_noise_conditional(self, xh_lig, eps, xh_pocket, lig_mask, pocket_mask, gamma):
+        """q(z_t | x, h) with the ligand COM removed from z and pocket (:162-183) as one dsb_ddpm_ligand_update launch:
+        coef = (1/alpha, 0, sigma) turns its z/alpha_ts - coef1 eps_hat + sigma noise into alpha xh + sigma eps."""
+        lib = _native.load()
+        alpha, sigma = self.alpha(gamma, gamma), self.sigma(gamma, gamma)
+        coef = torch.cat([1. / alpha, torch.zeros_like(alpha), sigma], dim=1).float().contiguous()
+        z, pocket_out = torch.empty_like(xh_lig), torch.empty_like(xh_pocket)
+        _native.check(lib.dsb_ddpm_ligand_update(
+            xh_lig.data_ptr(), eps.data_ptr(), eps.data_ptr(), coef.data_ptr(), lig_mask.data_ptr(), pocket_mask.data_ptr(),
+            xh_pocket.data_ptr(), len(lig_mask), len(pocket_mask), coef.shape[0], self.atom_nf, self.residue_nf,
+            z.data_ptr(), pocket_out.data_ptr(), C.c_void_p(torch.cuda.current_stream(xh_lig.device).cuda_stream)))
+        return z, pocket_out
+
+    @torch.no_grad()
+    def forward(self, ligand, pocket, return_info=False):
+        """Eval-mode variational bound (conditional_model.py:202-330): the terms of -log p(x, h | N, pocket) of the ligand
+        at one random t in [1, T] plus the t = 0 reconstruction term, with the reference's RNG call order (randint for t,
+        noise at t, noise at 0).  Training (t = 0 sampling, autograd) is not built."""
+        if self.training:
+            raise NotImplementedError('the training loss is not built (no backward kernels); call eval() for the NLL bound')
+        ligand, pocket = self.normalize(ligand, pocket)
+        lm, pm = ligand['mask'], pocket['mask']
+        n, device, nd = ligand['size'].size(0), ligand['x'].device, self.n_dims
+        delta_log_px = self.delta_log_px(ligand['size'])
+        t_int = torch.randint(1, self.T + 1, size=(n, 1), device=device).float()
+        s, t = (t_int - 1) / self.T, t_int / self.T
+        t_0 = torch.zeros_like(s)
+        gamma_s = self.inflate_batch_array(self.gamma(s), ligand['x'])
+        gamma_t = self.inflate_batch_array(self.gamma(t), ligand['x'])
+        gamma_0 = self.inflate_batch_array(self.gamma(t_0), ligand['x'])
+        xh0_lig = torch.cat([ligand['x'], ligand['one_hot']], dim=1)
+        xh0_pocket = torch.cat([pocket['x'], pocket['one_hot']], dim=1)
+        xh0_lig[:, :nd], xh0_pocket[:, :nd] = self.remove_mean_batch(xh0_lig[:, :nd], xh0_pocket[:, :nd], lm, pm)
+        SNR_weight = (1 - self.SNR(gamma_s - gamma_t)).squeeze(1)
+        neg_log_constants = -self.log_constants_p_x_given_z0(n_nodes=ligand['size'], device=device)
+
+        if self._vlb_native(device):
+            size = (len(lm), nd + self.atom_nf)
+            eps_t_lig = self.sample_gaussian(size=size, device=device)
+            z_t = self._native_noise_conditional(xh0_lig, eps_t_lig, xh0_pocket, lm, pm, gamma_t)
+            eps_0_lig = self.sample_gaussian(size=size, device=device)
+            z_0 = self._native_noise_conditional(xh0_lig, eps_0_lig, xh0_pocket, lm, pm, gamma_0)
+            (net_t_lig, _), (net_0_lig, _) = self._native_denoise_pair(z_t, t, z_0, t_0, lm, pm)
+            terms, xh_lig_hat = self._native_vlb_terms(
+                (xh0_lig, z_t[0], eps_t_lig, net_t_lig, z_0[0], eps_0_lig, net_0_lig), None, lm, pm, gamma_t, gamma_0,
+                self.vnode_idx)
+            error_t_lig = terms[:, 0]
+            loss_0_x_ligand, loss_0_h = 0.5 * terms[:, 2], -terms[:, 4]
+            kl_prior = self._kl_prior_from_norms(terms[:, 5], terms[:, 6], ligand['size'], device)
+            cnt = ligand['size'].clamp(min=1).float()
+            info = {'eps_hat_lig_x': (terms[:, 7] / (nd * cnt)).mean(),
+                    'eps_hat_lig_h': (terms[:, 8] / (self.atom_nf * cnt)).mean()}
+        else:
+            z_t_lig, xh_pocket_t, eps_t_lig = self.noised_representation(xh0_lig, xh0_pocket, lm, pm, gamma_t)
+            net_t_lig, _ = self.dynamics(z_t_lig, xh_pocket_t, t, lm, pm)
+            xh_lig_hat = self.xh_given_zt_and_epsilon(z_t_lig, net_t_lig, gamma_t, lm)
+            sq = (eps_t_lig - net_t_lig) ** 2
+            if self.vnode_idx is not None:
+                sq[self._virtual_rows(ligand), :nd] = 0
+            error_t_lig = self.sum_except_batch(sq, lm)
+            kl_prior = self.kl_prior(xh0_lig, lm, ligand['size'])
+            z_0_lig, xh_pocket_0, eps_0_lig = self.noised_representation(xh0_lig, xh0_pocket, lm, pm, gamma_0)
+            net_0_lig, _ = self.dynamics(z_0_lig, xh_pocket_0, t_0, lm, pm)
+            log_px, log_ph = self.log_pxh_given_z0_without_constants(ligand, z_0_lig, eps_0_lig, net_0_lig, gamma_0)
+            loss_0_x_ligand, loss_0_h = -log_px, -log_ph
+            info = {'eps_hat_lig_x': self._eps_hat_mean(net_t_lig[:, :nd], lm, n),
+                    'eps_hat_lig_h': self._eps_hat_mean(net_t_lig[:, nd:], lm, n)}
+
+        log_pN = self.log_pN(ligand['size'], pocket['size'])
+        terms = (delta_log_px, error_t_lig, torch.tensor(0.0), SNR_weight, loss_0_x_ligand, torch.tensor(0.0), loss_0_h,
+                 neg_log_constants, kl_prior, log_pN, t_int.squeeze(), xh_lig_hat)
+        return (*terms, info) if return_info else terms
+
     def partially_noised_ligand(self, ligand, pocket, noising_steps):
         """conditional_model.py:332-362."""
         t = torch.ones(size=(ligand['size'].size(0), 1), device=ligand['x'].device).float() * noising_steps / self.T
@@ -452,6 +552,17 @@ class SimpleConditionalDDPM(ConditionalDDPM):
 
     def _use_graph(self, device) -> bool:
         return False    # the fused update kernel hard-wires the COM projection of ConditionalDDPM
+
+    def _native_noise_conditional(self, xh_lig, eps, xh_pocket, lig_mask, pocket_mask, gamma):
+        z_lig, _ = self._native_noise(xh_lig, eps, None, None, lig_mask, pocket_mask, gamma)   # no COM projection
+        return z_lig, xh_pocket
+
+    def forward(self, ligand, pocket, return_info=False):
+        """conditional_model.py:727-735: the likelihood is evaluated in the frame of the pocket's centre of mass."""
+        pocket_com = scatter_mean(pocket['x'], pocket['mask'], dim=0)
+        ligand['x'] = ligand['x'] - pocket_com[ligand['mask']]
+        pocket['x'] = pocket['x'] - pocket_com[pocket['mask']]
+        return super().forward(ligand, pocket, return_info)
 
     @torch.no_grad()
     def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None):

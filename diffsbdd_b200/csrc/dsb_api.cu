@@ -638,6 +638,112 @@ __global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
   }
 }
 
+// ---- evaluation-mode variational bound (ConditionalDDPM / EnVariationalDiffusion.forward, eval branch) ----------------
+// z = alpha[g] xh + sigma[g] eps for ligand rows and (optional) pocket rows: q(z_t | x, h) of the joint model
+// (en_diffusion.py:302-317, eps.x already COM-free) and of SimpleConditionalDDPM (no COM projection, :702-735).
+__global__ void __launch_bounds__(128) ddpm_noise_kernel(const float* __restrict__ xl, const float* __restrict__ el,
+                                                          const float* __restrict__ xp, const float* __restrict__ ep,
+                                                          const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms,
+                                                          const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R,
+                                                          float* __restrict__ zl, float* __restrict__ zp) {
+  const int g = blockIdx.x;
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
+  const int D = 3 + A, DR = 3 + R;
+  const float alpha = coef[g * 2 + 0], sigma = coef[g * 2 + 1];
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) zl[idx] = alpha * xl[idx] + sigma * el[idx];
+  if (!xp) return;
+  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) zp[idx] = alpha * xp[idx] + sigma * ep[idx];
+}
+
+// log p(h | z_0) of one node (en_diffusion.py:216-255): discretised Gaussian around the un-normalised z_0.h, normalised
+// over the classes by log-sum-exp, dotted with the un-normalised one-hot.  zh / oh point at the node's h columns.
+__device__ __forceinline__ float vlb_log_ph(const float* zh, const float* oh, int K, float nv, float nb, float s0) {
+  auto lp = [&](int c) {
+    const float ctr = (zh[c] * nv + nb) - 1.f;
+    const float hi = 0.5f * (1.f + erff(((ctr + 0.5f) / s0) / 1.41421356237309515f));
+    const float lo = 0.5f * (1.f + erff(((ctr - 0.5f) / s0) / 1.41421356237309515f));
+    return logf(hi - lo + 1e-10f);
+  };
+  float m = -INFINITY, se = 0.f;                // online log-sum-exp
+  for (int c = 0; c < K; ++c) {
+    const float v = lp(c);
+    if (v > m) { se = se * expf(m - v) + 1.f; m = v; } else { se += expf(v - m); }
+  }
+  const float logz = m + logf(se);
+  float dot = 0.f;
+  for (int c = 0; c < K; ++c) dot += (lp(c) - logz) * (oh[c] * nv + nb);
+  return dot;
+}
+
+// Per-graph sums of the eval-mode loss; one block per graph, fixed summation order (no atomics), see
+// include/diffsbdd_b200.h for the column layout.  The pocket pointers are all NULL for the conditional model.
+__global__ void __launch_bounds__(128) ddpm_vlb_terms_kernel(
+    const float* __restrict__ xl, const float* __restrict__ ztl, const float* __restrict__ etl, const float* __restrict__ ntl,
+    const float* __restrict__ z0l, const float* __restrict__ e0l, const float* __restrict__ n0l,
+    const float* __restrict__ xp, const float* __restrict__ etp, const float* __restrict__ ntp,
+    const float* __restrict__ z0p, const float* __restrict__ e0p, const float* __restrict__ n0p,
+    const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res,
+    int NL, int NP, int A, int R, float nv, float nb, int vnode, float* __restrict__ terms, float* __restrict__ xh_hat) {
+  const int g = blockIdx.x;
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
+  const int D = 3 + A, DR = 3 + R;
+  const float alpha_T = coef[g * 4 + 0], s0 = coef[g * 4 + 1], alpha_t = coef[g * 4 + 2], sigma_t = coef[g * 4 + 3];
+  __shared__ float red[DSB_VLB_TERMS][4];
+  float v[DSB_VLB_TERMS];
+#pragma unroll
+  for (int k = 0; k < DSB_VLB_TERMS; ++k) v[k] = 0.f;
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const int c = idx % D, i = idx / D;
+    const float d = etl[idx] - ntl[idx];
+    const float mu = alpha_T * xl[idx];
+    xh_hat[idx] = ztl[idx] / alpha_t - ntl[idx] * sigma_t / alpha_t;       // en_diffusion.py:471-477
+    if (c < 3) {
+      const bool virt = vnode >= 0 && xl[(size_t)i * D + 3 + vnode] != 0.f;  // conditional_model.py:76-78, :264-266
+      const float d0 = e0l[idx] - n0l[idx];
+      if (!virt) { v[0] += d * d; v[2] += d0 * d0; }
+      v[5] += mu * mu;
+      v[7] += fabsf(ntl[idx]);
+    } else {
+      v[0] += d * d;
+      v[6] += mu * mu;
+      v[8] += fabsf(ntl[idx]);
+    }
+  }
+  for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x)
+    v[4] += vlb_log_ph(z0l + (size_t)i * D + 3, xl + (size_t)i * D + 3, A, nv, nb, s0);
+  if (xp) {
+    for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+      const int c = idx % DR;
+      const float d = etp[idx] - ntp[idx];
+      const float mu = alpha_T * xp[idx];
+      v[1] += d * d;
+      if (c < 3) {
+        const float d0 = e0p[idx] - n0p[idx];
+        v[3] += d0 * d0;
+        v[5] += mu * mu;
+        v[9] += fabsf(ntp[idx]);
+      } else {
+        v[6] += mu * mu;
+        v[10] += fabsf(ntp[idx]);
+      }
+    }
+    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x)
+      v[4] += vlb_log_ph(z0p + (size_t)i * DR + 3, xp + (size_t)i * DR + 3, R, nv, nb, s0);
+  }
+#pragma unroll
+  for (int k = 0; k < DSB_VLB_TERMS; ++k)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+  if ((threadIdx.x & 31) == 0)
+#pragma unroll
+    for (int k = 0; k < DSB_VLB_TERMS; ++k) red[k][threadIdx.x >> 5] = v[k];
+  __syncthreads();
+  if (threadIdx.x < DSB_VLB_TERMS) {
+    const int k = threadIdx.x;
+    terms[(size_t)g * DSB_VLB_TERMS + k] = (red[k][0] + red[k][1]) + (red[k][2] + red[k][3]);
+  }
+}
+
 }  // namespace dsb
 
 using namespace dsb;
@@ -958,6 +1064,49 @@ int dsb_ddpm_joint_inpaint_update(float* z_lig, float* z_pocket, const float* xh
   ddpm_joint_inpaint_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
       z_lig, z_pocket, xh0_lig, xh0_pocket, lig_fixed, pocket_fixed, noise_x, noise_h_lig, noise_h_pocket, renoise_x, renoise_h_lig,
       renoise_h_pocket, coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_noise(const float* xh_lig, const float* eps_lig, const float* xh_pocket, const float* eps_pocket,
+                   const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms,
+                   int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, float* z_lig, float* z_pocket,
+                   void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!xh_lig || !eps_lig || !coef || !mask_atoms || !mask_residues || !z_lig ||
+      (xh_pocket && (!eps_pocket || !z_pocket))) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  if (int rc = check_sizes(n_atoms, n_residues, n_graphs, 0)) return rc;
+  ddpm_noise_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(xh_lig, eps_lig, xh_pocket, eps_pocket, coef, mask_atoms,
+                                                                         mask_residues, (int)n_atoms, (int)n_residues, atom_nf,
+                                                                         residue_nf, z_lig, z_pocket);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_vlb_terms(const float* xh0_lig, const float* z_t_lig, const float* eps_t_lig, const float* net_t_lig,
+                       const float* z_0_lig, const float* eps_0_lig, const float* net_0_lig, const float* xh0_pocket,
+                       const float* eps_t_pocket, const float* net_t_pocket, const float* z_0_pocket, const float* eps_0_pocket,
+                       const float* net_0_pocket, const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues,
+                       int64_t n_atoms, int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf,
+                       float norm_value_h, float norm_bias_h, int32_t vnode_idx, float* terms, float* xh_lig_hat, void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!xh0_lig || !z_t_lig || !eps_t_lig || !net_t_lig || !z_0_lig || !eps_0_lig || !net_0_lig || !coef || !mask_atoms ||
+      !mask_residues || !terms || !xh_lig_hat ||
+      (xh0_pocket && (!eps_t_pocket || !net_t_pocket || !z_0_pocket || !eps_0_pocket || !net_0_pocket))) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  if (int rc = check_sizes(n_atoms, n_residues, n_graphs, 0)) return rc;
+  if (atom_nf <= 0 || residue_nf <= 0 || vnode_idx >= atom_nf || !(norm_value_h > 0.f)) {
+    set_error("dsb_ddpm_vlb_terms: bad atom_nf=%d residue_nf=%d vnode_idx=%d norm_value_h=%g", atom_nf, residue_nf, vnode_idx,
+              (double)norm_value_h);
+    return DSB_ERR_INVALID_ARGUMENT;
+  }
+  ddpm_vlb_terms_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
+      xh0_lig, z_t_lig, eps_t_lig, net_t_lig, z_0_lig, eps_0_lig, net_0_lig, xh0_pocket, eps_t_pocket, net_t_pocket, z_0_pocket,
+      eps_0_pocket, net_0_pocket, coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, norm_value_h,
+      norm_bias_h, vnode_idx, terms, xh_lig_hat);
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -3,8 +3,9 @@
 reference: equivariant_diffusion/en_diffusion.py.  Only what the sampling path needs is built: noise
 schedule (:1105-1190), alpha/sigma helpers (:83-107, :865-878), (un)normalisation (:880-912), COM helpers
 (:919-930), node-count prior (:958-1000), ``sample_p_zs_given_zt`` (:503-557), ``sample_p_xh_given_z0``
-(:263-288), ``sample`` (:581-651).  Loss/likelihood members (``forward``, ``kl_prior``, ``log_pxh_...``)
-raise NotImplementedError — training is out of scope (SURVEY.md §8).
+(:263-288), ``sample`` (:581-651), and the eval-mode likelihood ``forward`` (:336-469) with its helpers (``kl_prior_with_pocket``,
+``log_pxh_given_z0_without_constants``, ``log_constants_p_x_given_z0``, ``gaussian_KL``, ``log_pN``, ``delta_log_px``).
+Training (``forward`` in train mode, autograd) raises NotImplementedError.
 
 Class and attribute names are the reference's, so ``LigandPocketDDPM.generate_ligands``'s exact-type
 dispatch (lightning_modules.py:814, :837) and Lightning checkpoints (keys ``ddpm.gamma.gamma``,
@@ -151,6 +152,12 @@ class DistributionNodes:
         assert (n1 is None) ^ (n2 is None), "Exactly one input argument must be None"
         dists, cond = (self.n1_given_n2, n2) if n2 is not None else (self.n2_given_n1, n1)
         return torch.tensor([dists[int(i)].sample() for i in cond], device=cond.device)
+
+    def log_prob(self, batch_n_nodes_1, batch_n_nodes_2):
+        """en_diffusion.py:1002-1014: log p(n_ligand, n_pocket) under the joint histogram."""
+        assert batch_n_nodes_1.dim() == 1 and batch_n_nodes_2.dim() == 1
+        idx = torch.tensor([self.n_nodes_to_idx[pair] for pair in zip(batch_n_nodes_1.tolist(), batch_n_nodes_2.tolist())])
+        return self.m.log_prob(idx).to(batch_n_nodes_1.device)
 
     def log_prob_n1_given_n2(self, n1, n2):
         return torch.stack([self.n1_given_n2[int(c)].log_prob(i.cpu()) for i, c in zip(n1, n2)]).to(n1.device)
@@ -654,6 +661,194 @@ class EnVariationalDiffusion(nn.Module):
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lmask, pmask
 
-    # ---- training-side members: out of scope ----------------------------------------------------------------
+    # ---- evaluation-mode variational bound (en_diffusion.py:109-261, :319-469) ---------------------------------------
+    @staticmethod
+    def gaussian_KL(q_mu_minus_p_mu_squared, q_sigma, p_sigma, d):
+        """KL(N(mu_q, q_sigma^2 I_d) || N(mu_p, p_sigma^2 I_d)) from ||mu_q - mu_p||^2 (en_diffusion.py:840-853)."""
+        log_ratio = torch.log(p_sigma / q_sigma)
+        return d * log_ratio + 0.5 * (d * q_sigma ** 2 + q_mu_minus_p_mu_squared) / (p_sigma ** 2) - 0.5 * d
+
+    @staticmethod
+    def cdf_standard_gaussian(x):
+        return 0.5 * (1. + torch.erf(x / math.sqrt(2)))
+
+    def log_pN(self, N_lig, N_pocket):
+        """log p(N) of the joint size prior, so that -log p(x, h, N) = -log p(x, h | N) - log p(N)."""
+        return self.size_distribution.log_prob(N_lig, N_pocket)
+
+    def delta_log_px(self, num_nodes):
+        """Log-volume change of the coordinate normalisation x / norm_values[0] on the x subspace."""
+        return -self.subspace_dimensionality(num_nodes) * np.log(self.norm_values[0])
+
+    def log_constants_p_x_given_z0(self, n_nodes, device):
+        """The sigma_0-dependent constants of log p(x | z_0): sigma_x = SNR(-gamma_0 / 2) per dimension."""
+        n = len(n_nodes)
+        dof = self.subspace_dimensionality(n_nodes)
+        log_sigma_x = 0.5 * self.gamma(torch.zeros((n, 1), device=device)).view(n)
+        return dof * (-log_sigma_x - 0.5 * np.log(2 * np.pi))
+
+    def _kl_prior_from_norms(self, mu_norm2_x, mu_norm2_h, num_nodes, device):
+        """KL(q(z_T | x, h) || N(0, I)) from ||alpha_T x||^2 and ||alpha_T h||^2 per graph."""
+        gamma_T = self.gamma(torch.ones((len(num_nodes), 1), device=device))
+        sigma_T = self.sigma(gamma_T, gamma_T).view(-1)
+        ones = torch.ones_like(sigma_T)
+        kl_h = self.gaussian_KL(mu_norm2_h, sigma_T, ones, d=1)
+        kl_x = self.gaussian_KL(mu_norm2_x, sigma_T, ones, self.subspace_dimensionality(num_nodes))
+        return kl_x + kl_h
+
+    def kl_prior_with_pocket(self, xh_lig, xh_pocket, mask_lig, mask_pocket, num_nodes):
+        """en_diffusion.py:109-155: KL of q(z_T | x, h) of ligand and pocket against the standard normal prior."""
+        nd = self.n_dims
+        alpha_T = self.alpha(self.gamma(torch.ones((len(num_nodes), 1), device=xh_lig.device)), xh_lig)
+        mu_lig, mu_pocket = alpha_T[mask_lig] * xh_lig, alpha_T[mask_pocket] * xh_pocket
+        norm_x = self.sum_except_batch(mu_lig[:, :nd] ** 2, mask_lig) + self.sum_except_batch(mu_pocket[:, :nd] ** 2, mask_pocket)
+        norm_h = self.sum_except_batch(mu_lig[:, nd:] ** 2, mask_lig) + self.sum_except_batch(mu_pocket[:, nd:] ** 2, mask_pocket)
+        return self._kl_prior_from_norms(norm_x, norm_h, num_nodes, xh_lig.device)
+
+    def _log_ph_given_z0(self, one_hot, z_h, sigma_0_cat, mask, epsilon=1e-10):
+        """Discretised-Gaussian likelihood of the one-hot types given z_0.h, summed per graph (en_diffusion.py:216-255)."""
+        target = one_hot * self.norm_values[1] + self.norm_biases[1]
+        centred = (z_h * self.norm_values[1] + self.norm_biases[1]) - 1
+        width = sigma_0_cat[mask]
+        log_p = torch.log(self.cdf_standard_gaussian((centred + 0.5) / width)
+                          - self.cdf_standard_gaussian((centred - 0.5) / width) + epsilon)
+        log_p = log_p - torch.logsumexp(log_p, dim=1, keepdim=True)
+        return self.sum_except_batch(log_p * target, mask)
+
+    def log_pxh_given_z0_without_constants(self, ligand, z_0_lig, eps_lig, net_out_lig, pocket, z_0_pocket, eps_pocket,
+                                           net_out_pocket, gamma_0, epsilon=1e-10):
+        """en_diffusion.py:185-261: -1/2 |eps_0.x - net_0.x|^2 of ligand and pocket, and log p(h | z_0) of both."""
+        nd = self.n_dims
+        sigma_0_cat = self.sigma(gamma_0, target_tensor=z_0_lig) * self.norm_values[1]
+        log_px_lig = -0.5 * self.sum_except_batch((eps_lig[:, :nd] - net_out_lig[:, :nd]) ** 2, ligand['mask'])
+        log_px_pocket = -0.5 * self.sum_except_batch((eps_pocket[:, :nd] - net_out_pocket[:, :nd]) ** 2, pocket['mask'])
+        log_ph = self._log_ph_given_z0(ligand['one_hot'], z_0_lig[:, nd:], sigma_0_cat, ligand['mask'], epsilon) + \
+            self._log_ph_given_z0(pocket['one_hot'], z_0_pocket[:, nd:], sigma_0_cat, pocket['mask'], epsilon)
+        return log_px_lig, log_px_pocket, log_ph
+
+    @staticmethod
+    def _eps_hat_mean(net_out, mask, n_graphs):
+        """Mean over graphs of the per-graph mean |net_out| (the ``info`` entries of forward)."""
+        return scatter_mean(net_out.abs().mean(1), mask, dim=0, dim_size=n_graphs).mean()
+
+    def _vlb_native(self, device) -> bool:
+        """Evaluation-mode forward on the native kernels: 'auto' on CUDA with the native EGNNDynamics; 'eager' keeps the
+        reference-order torch ops; 'graph' insists on the native path."""
+        from .dynamics import EGNNDynamics
+        if self.loop_engine == 'eager':
+            return False
+        ok = isinstance(self.dynamics, EGNNDynamics) and torch.device(device).type == 'cuda'
+        if self.loop_engine == 'graph' and not ok:
+            raise RuntimeError("loop_engine='graph' needs the native EGNNDynamics on a CUDA device")
+        return ok
+
+    def _native_denoise_pair(self, z_t, t, z_0, t_0, lig_mask, pocket_mask):
+        """The two denoiser calls of the eval forward (at t and at 0) with one NaN check after both."""
+        dyn = self.dynamics
+        prev, dyn.defer_status_check = dyn.defer_status_check, True
+        try:
+            net_t = dyn(z_t[0], z_t[1], t, lig_mask, pocket_mask)
+            net_0 = dyn(z_0[0], z_0[1], t_0, lig_mask, pocket_mask)
+        finally:
+            dyn.defer_status_check = prev
+        dyn.check_status()
+        return net_t, net_0
+
+    def _native_noise(self, xh_lig, eps_lig, xh_pocket, eps_pocket, lig_mask, pocket_mask, gamma):
+        """z = alpha xh + sigma eps per graph in one launch (libdiffsbdd_b200 dsb_ddpm_noise); pocket skipped if None."""
+        from . import _native
+        lib = _native.load()
+        coef = torch.cat([self.alpha(gamma, gamma), self.sigma(gamma, gamma)], dim=1).float().contiguous()
+        z_lig = torch.empty_like(xh_lig)
+        z_pocket = None if xh_pocket is None else torch.empty_like(xh_pocket)
+        ptr = lambda x: None if x is None else x.data_ptr()
+        _native.check(lib.dsb_ddpm_noise(
+            ptr(xh_lig), ptr(eps_lig), ptr(xh_pocket), ptr(eps_pocket), ptr(coef), ptr(lig_mask), ptr(pocket_mask),
+            len(lig_mask), len(pocket_mask), coef.shape[0], self.atom_nf, self.residue_nf, ptr(z_lig), ptr(z_pocket),
+            torch.cuda.current_stream(xh_lig.device).cuda_stream))
+        return z_lig, z_pocket
+
+    def _native_vlb_terms(self, lig, pocket, lig_mask, pocket_mask, gamma_t, gamma_0, vnode_idx):
+        """One dsb_ddpm_vlb_terms launch.  lig = (xh0, z_t, eps_t, net_t, z_0, eps_0, net_0); pocket = (xh0, eps_t, net_t, z_0,
+        eps_0, net_0) or None (ligand-only likelihood).  Returns the per-graph sums [n_graphs, 11] and xh_lig_hat."""
+        from . import _native
+        lib = _native.load()
+        n = gamma_t.shape[0]
+        device = lig[0].device
+        gamma_T = self.gamma(torch.ones((n, 1), device=device))
+        coef = torch.cat([self.alpha(gamma_T, gamma_T), self.sigma(gamma_0, gamma_0) * self.norm_values[1],
+                          self.alpha(gamma_t, gamma_t), self.sigma(gamma_t, gamma_t)], dim=1).float().contiguous()
+        lig = [x.float().contiguous() for x in lig]
+        pocket = [None] * 6 if pocket is None else [x.float().contiguous() for x in pocket]
+        terms = torch.empty((n, 11), device=device)
+        xh_lig_hat = torch.empty_like(lig[1])
+        ptr = lambda x: None if x is None else x.data_ptr()
+        _native.check(lib.dsb_ddpm_vlb_terms(
+            *[ptr(x) for x in lig], *[ptr(x) for x in pocket], ptr(coef), ptr(lig_mask), ptr(pocket_mask), len(lig_mask),
+            len(pocket_mask), n, self.atom_nf, self.residue_nf, float(self.norm_values[1]), float(self.norm_biases[1]),
+            -1 if vnode_idx is None else int(vnode_idx), ptr(terms), ptr(xh_lig_hat),
+            torch.cuda.current_stream(device).cuda_stream))
+        return terms, xh_lig_hat
+
+    @torch.no_grad()
     def forward(self, ligand, pocket, return_info=False):
-        raise NotImplementedError('training loss is out of scope of diffsbdd_b200 (sampling hot path only)')
+        """Eval-mode variational bound of the joint model (en_diffusion.py:336-469): the terms of -log p(x, h | N) for
+        ligand and pocket at one random t in [1, T] plus the t = 0 reconstruction term.  RNG calls as the reference:
+        randint for t, then the noise at t, then the noise at 0.  Training (t = 0 sampling, autograd) is not built."""
+        if self.training:
+            raise NotImplementedError('the training loss is not built (no backward kernels); call eval() for the NLL bound')
+        ligand, pocket = self.normalize(ligand, pocket)
+        lm, pm = ligand['mask'], pocket['mask']
+        n, device, nd = ligand['size'].size(0), ligand['x'].device, self.n_dims
+        n_nodes = ligand['size'] + pocket['size']
+        delta_log_px = self.delta_log_px(n_nodes)
+        t_int = torch.randint(1, self.T + 1, size=(n, 1), device=device).float()
+        s, t = (t_int - 1) / self.T, t_int / self.T
+        t_0 = torch.zeros_like(s)
+        gamma_s = self.inflate_batch_array(self.gamma(s), ligand['x'])
+        gamma_t = self.inflate_batch_array(self.gamma(t), ligand['x'])
+        gamma_0 = self.inflate_batch_array(self.gamma(t_0), ligand['x'])
+        xh_lig = torch.cat([ligand['x'], ligand['one_hot']], dim=1)
+        xh_pocket = torch.cat([pocket['x'], pocket['one_hot']], dim=1)
+        SNR_weight = (1 - self.SNR(gamma_s - gamma_t)).squeeze(1)
+        neg_log_constants = -self.log_constants_p_x_given_z0(n_nodes=n_nodes, device=device)
+
+        if self._vlb_native(device):
+            eps_t = self.sample_combined_position_feature_noise(lm, pm)
+            z_t = self._native_noise(xh_lig, eps_t[0], xh_pocket, eps_t[1], lm, pm, gamma_t)
+            eps_0 = self.sample_combined_position_feature_noise(lm, pm)
+            z_0 = self._native_noise(xh_lig, eps_0[0], xh_pocket, eps_0[1], lm, pm, gamma_0)
+            (net_t_lig, net_t_pocket), (net_0_lig, net_0_pocket) = self._native_denoise_pair(z_t, t, z_0, t_0, lm, pm)
+            terms, xh_lig_hat = self._native_vlb_terms(
+                (xh_lig, z_t[0], eps_t[0], net_t_lig, z_0[0], eps_0[0], net_0_lig),
+                (xh_pocket, eps_t[1], net_t_pocket, z_0[1], eps_0[1], net_0_pocket), lm, pm, gamma_t, gamma_0, None)
+            error_t_lig, error_t_pocket = terms[:, 0], terms[:, 1]
+            loss_0_x_ligand, loss_0_x_pocket, loss_0_h = 0.5 * terms[:, 2], 0.5 * terms[:, 3], -terms[:, 4]
+            kl_prior = self._kl_prior_from_norms(terms[:, 5], terms[:, 6], n_nodes, device)
+            cnt_l = ligand['size'].clamp(min=1).float()
+            cnt_p = pocket['size'].clamp(min=1).float()
+            info = {'eps_hat_lig_x': (terms[:, 7] / (nd * cnt_l)).mean(),
+                    'eps_hat_lig_h': (terms[:, 8] / (self.atom_nf * cnt_l)).mean(),
+                    'eps_hat_pocket_x': (terms[:, 9] / (nd * cnt_p)).mean(),
+                    'eps_hat_pocket_h': (terms[:, 10] / (self.residue_nf * cnt_p)).mean()}
+        else:
+            z_t_lig, z_t_pocket, eps_t_lig, eps_t_pocket = self.noised_representation(xh_lig, xh_pocket, lm, pm, gamma_t)
+            net_t_lig, net_t_pocket = self.dynamics(z_t_lig, z_t_pocket, t, lm, pm)
+            xh_lig_hat = self.xh_given_zt_and_epsilon(z_t_lig, net_t_lig, gamma_t, lm)
+            error_t_lig = self.sum_except_batch((eps_t_lig - net_t_lig) ** 2, lm)
+            error_t_pocket = self.sum_except_batch((eps_t_pocket - net_t_pocket) ** 2, pm)
+            kl_prior = self.kl_prior_with_pocket(xh_lig, xh_pocket, lm, pm, n_nodes)
+            z_0_lig, z_0_pocket, eps_0_lig, eps_0_pocket = self.noised_representation(xh_lig, xh_pocket, lm, pm, gamma_0)
+            net_0_lig, net_0_pocket = self.dynamics(z_0_lig, z_0_pocket, t_0, lm, pm)
+            log_px_lig, log_px_pocket, log_ph = self.log_pxh_given_z0_without_constants(
+                ligand, z_0_lig, eps_0_lig, net_0_lig, pocket, z_0_pocket, eps_0_pocket, net_0_pocket, gamma_0)
+            loss_0_x_ligand, loss_0_x_pocket, loss_0_h = -log_px_lig, -log_px_pocket, -log_ph
+            info = {'eps_hat_lig_x': self._eps_hat_mean(net_t_lig[:, :nd], lm, n),
+                    'eps_hat_lig_h': self._eps_hat_mean(net_t_lig[:, nd:], lm, n),
+                    'eps_hat_pocket_x': self._eps_hat_mean(net_t_pocket[:, :nd], pm, n),
+                    'eps_hat_pocket_h': self._eps_hat_mean(net_t_pocket[:, nd:], pm, n)}
+
+        log_pN = self.log_pN(ligand['size'], pocket['size'])
+        terms = (delta_log_px, error_t_lig, error_t_pocket, SNR_weight, loss_0_x_ligand, loss_0_x_pocket, loss_0_h,
+                 neg_log_constants, kl_prior, log_pN, t_int.squeeze(), xh_lig_hat)
+        return (*terms, info) if return_info else terms

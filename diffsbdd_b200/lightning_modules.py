@@ -4,8 +4,9 @@ reference: lightning_modules.py — constructor / model assembly (:31-173), ``pr
 ``generate_ligands`` (:754-872).  Kept: class name, constructor signature, ``load_from_checkpoint``,
 ``.ddpm`` (with the reference's DDPM class identities — ``generate_ligands`` dispatches on the exact type,
 lightning_modules.py:814, :837), ``.x_dims/.atom_nf/.aa_nf``, ``lig_type_encoder/decoder``,
-``pocket_type_encoder/decoder``, ``dataset_info``.  Not built (out of scope, SURVEY.md §2 rows 5-7, 12):
-training/validation steps, W&B logging, molecule metrics, visualisation.  PDB parsing (BioPython) and
+``pocket_type_encoder/decoder``, ``dataset_info``; the likelihood evaluation ``forward`` / ``validation_step`` /
+``test_step`` (:217-302, :365-380).  Not built (out of scope, SURVEY.md §2 rows 5-7, 12): training steps, W&B logging,
+molecule metrics, visualisation.  PDB parsing (BioPython) and
 molecule building (RDKit/OpenBabel, the reference's ``analysis`` package) are imported lazily and only by
 ``generate_ligands``; the tensor-level path ``generate_ligand_tensors`` needs neither.
 
@@ -75,6 +76,8 @@ class LigandPocketDDPM(_Base):
         self.mode, self.pocket_representation = mode, pocket_representation
         self.dataset_name, self.datadir, self.outdir = dataset, datadir, outdir
         self.batch_size, self.lr = batch_size, lr
+        self.loss_type = _get(diffusion_params, 'diffusion_loss_type')
+        self.auxiliary_loss = auxiliary_loss
         self.T = _get(diffusion_params, 'diffusion_steps')
         self.dataset_info = _dataset_info(dataset)
         self.lig_type_encoder = dict(self.dataset_info['atom_encoder'])
@@ -229,5 +232,57 @@ class LigandPocketDDPM(_Base):
                 molecules.append(mol)
         return molecules
 
+    # ---- likelihood evaluation (lightning_modules.py:217-302, :365-380) ---------------------------------------------
+    def get_ligand_and_pocket(self, data):
+        """Batch dict of the reference's datasets -> (ligand, pocket) dicts on this module's device."""
+        ligand = {'x': data['lig_coords'].to(self.device, FLOAT_TYPE),
+                  'one_hot': data['lig_one_hot'].to(self.device, FLOAT_TYPE),
+                  'size': data['num_lig_atoms'].to(self.device, INT_TYPE),
+                  'mask': data['lig_mask'].to(self.device, INT_TYPE)}
+        if self.virtual_nodes:
+            ligand['num_virtual_atoms'] = data['num_virtual_atoms'].to(self.device, INT_TYPE)
+        pocket = {'x': data['pocket_coords'].to(self.device, FLOAT_TYPE),
+                  'one_hot': data['pocket_one_hot'].to(self.device, FLOAT_TYPE),
+                  'size': data['num_pocket_nodes'].to(self.device, INT_TYPE),
+                  'mask': data['pocket_mask'].to(self.device, INT_TYPE)}
+        return ligand, pocket
+
     def forward(self, data):
-        raise NotImplementedError('training is out of scope of diffsbdd_b200')
+        """Per-complex negative log-likelihood bound -log p(x, h, N) (the VLB / evaluation branch of the reference) and the
+        batch means of its terms.  Training (the l2 loss, the Lennard-Jones auxiliary term) is not built."""
+        if self.training:
+            raise NotImplementedError('training is not built in diffsbdd_b200 (no backward kernels); call eval() first')
+        ligand, pocket = self.get_ligand_and_pocket(data)
+        delta_log_px, error_t_lig, error_t_pocket, SNR_weight, loss_0_x_ligand, loss_0_x_pocket, loss_0_h, \
+            neg_log_const_0, kl_prior, log_pN, _t_int, _xh_lig_hat, info = self.ddpm(ligand, pocket, return_info=True)
+        # the loss terms are negative log-likelihoods; SNR_weight = 1 - SNR(s - t) is negative
+        loss_t = -self.T * 0.5 * SNR_weight * (error_t_lig + error_t_pocket)
+        loss_0 = loss_0_x_ligand + loss_0_x_pocket + loss_0_h + neg_log_const_0
+        nll = loss_t + loss_0 + kl_prior - delta_log_px
+        if not self.virtual_nodes:          # -log p(x, h, N) = -log p(x, h | N) - log p(N); constant N with virtual nodes
+            nll = nll - log_pN
+        for key, val in (('error_t_lig', error_t_lig), ('error_t_pocket', error_t_pocket), ('SNR_weight', SNR_weight),
+                         ('loss_0', loss_0), ('kl_prior', kl_prior), ('delta_log_px', delta_log_px),
+                         ('neg_log_const_0', neg_log_const_0), ('log_pN', log_pN)):
+            info[key] = val.mean(0)
+        return nll, info
+
+    def log_metrics(self, metrics_dict, split, batch_size=None, **kwargs):
+        if pl is None or getattr(self, '_trainer', None) is None:
+            return                          # logging needs a Lightning trainer
+        for m, value in metrics_dict.items():
+            self.log(f'{m}/{split}', value, batch_size=batch_size, **kwargs)
+
+    def _shared_eval(self, data, prefix, *args):
+        nll, info = self.forward(data)
+        info['loss'] = nll.mean(0)
+        self.log_metrics(info, prefix, batch_size=len(data['num_lig_atoms']), sync_dist=True)
+        return info
+
+    @torch.no_grad()
+    def validation_step(self, data, *args):
+        return self._shared_eval(data, 'val', *args)
+
+    @torch.no_grad()
+    def test_step(self, data, *args):
+        return self._shared_eval(data, 'test', *args)

@@ -144,6 +144,23 @@ def synthetic_pocket(cfg: DynamicsConfig, n_pocket, seed: int = 0, density: floa
     }
 
 
+def synthetic_complex_batch(cfg: DynamicsConfig, n_lig, n_pocket, seed: int = 0, density: float = 0.045,
+                            lig_sigma: float = 1.5) -> Dict[str, torch.Tensor]:
+    """A batch dict with the keys of the reference datasets (lightning_modules.py:217-234) for likelihood evaluation:
+    ``synthetic_pocket`` pockets with ligands ~ N(pocket COM, lig_sigma^2) and random atom types."""
+    p = synthetic_pocket(cfg, n_pocket, seed=seed, density=density)
+    g = torch.Generator(device='cpu')
+    g.manual_seed(_key_seed('ligand', seed))
+    sizes = torch.tensor(list(n_lig), dtype=torch.int64)
+    mask = torch.repeat_interleave(torch.arange(len(sizes)), sizes)
+    com = torch.zeros((len(sizes), 3)).index_add_(0, p['mask'], p['x']) / p['size'].clamp(min=1).unsqueeze(1).float()
+    x = com[mask] + lig_sigma * torch.randn((len(mask), 3), generator=g)
+    types = torch.randint(0, cfg.atom_nf, (len(mask),), generator=g)
+    return {'lig_coords': x, 'lig_one_hot': torch.nn.functional.one_hot(types, cfg.atom_nf).float(),
+            'num_lig_atoms': sizes, 'lig_mask': mask, 'pocket_coords': p['x'], 'pocket_one_hot': p['one_hot'],
+            'num_pocket_nodes': p['size'], 'pocket_mask': p['mask']}
+
+
 def synthetic_denoiser_inputs(cfg: DynamicsConfig, n_lig, n_pocket, seed: int = 0,
                               density: float = 0.045, t_value=None,
                               norm_values=(1.0, 4.0), lig_sigma: float = 1.0):

@@ -202,6 +202,43 @@ int dsb_ddpm_joint_inpaint_update(float* z_lig, float* z_pocket, const float* xh
                                   int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf,
                                   void* stream);
 
+/* ---- evaluation-mode variational bound (validation / test NLL): what EnVariationalDiffusion.forward, ConditionalDDPM.forward
+ * and SimpleConditionalDDPM.forward compute in eval mode besides the two denoiser calls and the per-graph scalar algebra.
+ *
+ * dsb_ddpm_noise = q(z_t | x, h) without a COM projection (en_diffusion.py:302-317; SimpleConditionalDDPM, conditional_model.py:702-735):
+ *   z_lig = alpha[g] xh_lig + sigma[g] eps_lig ;  z_pocket = alpha[g] xh_pocket + sigma[g] eps_pocket (skipped if xh_pocket == NULL).
+ * coef [n_graphs, 2] = (alpha_t, sigma_t).  For the joint model eps.x must already be COM-free over ligand + pocket.
+ * (ConditionalDDPM noises with dsb_ddpm_ligand_update and coef = (1/alpha_t, 0, sigma_t): z = xh/(1/alpha) + sigma eps, ligand COM
+ * removed from z and pocket, conditional_model.py:162-183.)
+ *
+ * dsb_ddpm_vlb_terms: one block per graph over the row ranges of the sorted masks, fixed summation order (no atomics), so `terms`
+ * repeats bit for bit for identical inputs.  Inputs [rows, 3+nf] fp32:
+ *   xh0_*   the normalised data x (as noised) | h = (one_hot - norm_bias_h) / norm_value_h ; its h columns are the one-hot
+ *   z_t_lig, eps_t_*, net_t_*   noised sample, noise and denoiser output at the random t
+ *   z_0_*,   eps_0_*, net_0_*   the same at t = 0
+ * The pocket pointers are all NULL for the conditional models (ligand-only likelihood).
+ * coef [n_graphs, 4] = (alpha_T, sigma_0 * norm_value_h, alpha_t, sigma_t).  vnode_idx: ligand class of virtual atoms (-1 = none);
+ * the x columns of ligand rows whose h column vnode_idx is non-zero are left out of columns 0 and 2 (conditional_model.py:76-78).
+ * terms [n_graphs, DSB_VLB_TERMS], per graph:
+ *   0 sum (eps_t - net_t)^2 ligand (all columns)         1 the same, pocket                     -> error_t (:262-267, en_diffusion.py:385-390)
+ *   2 sum (eps_0.x - net_0.x)^2 ligand                   3 the same, pocket                     -> -2 log p(x | z_0) w/o constants
+ *   4 log p(h | z_0), ligand + pocket: sum over nodes of one_hot . (log(Phi((c+1/2)/s0) - Phi((c-1/2)/s0) + 1e-10) - logsumexp),
+ *     c = z_0.h * norm_value_h + norm_bias_h - 1, Phi(x) = (1 + erf(x / sqrt 2)) / 2, one_hot un-normalised (en_diffusion.py:185-261)
+ *   5 |alpha_T x|^2, ligand + pocket   6 |alpha_T h|^2, ligand + pocket                          -> kl_prior (en_diffusion.py:109-155)
+ *   7 sum |net_t.x| ligand   8 sum |net_t.h| ligand   9 sum |net_t.x| pocket   10 sum |net_t.h| pocket  -> the info means (:451-464)
+ * xh_lig_hat [n_atoms, 3+atom_nf] = z_t / alpha_t - net_t * sigma_t / alpha_t (en_diffusion.py:471-477). */
+#define DSB_VLB_TERMS 11
+int dsb_ddpm_noise(const float* xh_lig, const float* eps_lig, const float* xh_pocket, const float* eps_pocket,
+                   const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms,
+                   int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, float* z_lig, float* z_pocket,
+                   void* stream);
+int dsb_ddpm_vlb_terms(const float* xh0_lig, const float* z_t_lig, const float* eps_t_lig, const float* net_t_lig,
+                       const float* z_0_lig, const float* eps_0_lig, const float* net_0_lig, const float* xh0_pocket,
+                       const float* eps_t_pocket, const float* net_t_pocket, const float* z_0_pocket, const float* eps_0_pocket,
+                       const float* net_0_pocket, const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues,
+                       int64_t n_atoms, int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf,
+                       float norm_value_h, float norm_bias_h, int32_t vnode_idx, float* terms, float* xh_lig_hat, void* stream);
+
 const char* dsb_last_error(void);
 const char* dsb_version(void);
 
