@@ -210,8 +210,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
         def reset():
             st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
 
-        # warm-up on a side stream (allocator + plan caches + workspace), restoring RNG and state afterwards
+        # warm-up on a side stream (allocator + plan caches + workspace), restoring RNG and state afterwards.  It runs on the
+        # real inputs: the static buffers start uninitialised, and a NaN left there by an earlier allocation would set the
+        # sticky NaN flag that the deferred status check reports after the loop.
         rng = torch.cuda.get_rng_state(device)
+        reset()
         side = torch.cuda.Stream(device=device)
         side.wait_stream(torch.cuda.current_stream(device))
         with torch.cuda.stream(side):

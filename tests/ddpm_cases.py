@@ -1,4 +1,6 @@
 """Shared definitions of the DDPM-wrapper parity cases (used by the golden generator and the tests)."""
+import math
+
 import torch
 
 from diffsbdd_b200.config import DynamicsConfig
@@ -62,3 +64,29 @@ def make_ligand(n_lig, n_fixed, device='cpu'):
     lig = {'x': x.to(device), 'one_hot': torch.nn.functional.one_hot(types, DDPM_CFG.atom_nf).float().to(device),
            'size': torch.tensor(n_lig, device=device), 'mask': mask.to(device)}
     return lig, fixed.to(device)
+
+
+# per-graph (ligand rows, pocket rows) of the fused-kernel tests: each test's own small ragged batch, the configs[2] batch, and
+# a batch with more than 128 ligand rows and 300 pocket rows in one graph (one 128-thread block per graph: strided row loops)
+# next to a one-atom ligand
+DDPM_SHAPES = {
+    'ragged': None,
+    'configs2': ([25] * 64, [175] * 64),
+    'large': ([150, 1, 20], [300, 40, 9]),
+}
+
+
+def ddpm_shape(shape, ragged_lig, ragged_poc):
+    return (ragged_lig, ragged_poc) if DDPM_SHAPES[shape] is None else DDPM_SHAPES[shape]
+
+
+def assert_fp64_bound(got, want32, want64, what):
+    """The kernel's max-abs error against the float64 evaluation of the same ops on the same fp32 inputs is at most twice the
+    error of the fp32 torch ops, or 4 ulp of the output's largest magnitude, whichever is larger."""
+    got, want32, want64 = (x.detach().cpu().double() for x in (got, want32, want64))
+    err = float((got - want64).abs().max())
+    err32 = float((want32 - want64).abs().max())
+    big = float(want64.abs().max())
+    ulp = 2.0 ** (math.floor(math.log2(big)) - 23) if big > 0 else 0.0
+    bound = max(2.0 * err32, 4.0 * ulp)
+    assert err <= bound, f'{what}: kernel error {err:.3e} vs float64 > {bound:.3e} (fp32 torch ops {err32:.3e}, 4 ulp {4 * ulp:.3e})'

@@ -82,6 +82,10 @@ CASES = {
     'sin_h256_l2': (DynamicsConfig(n_layers=2, sin_embedding=True), [12, 9], [40, 33], 29, 13, 0.045, None, (1.0, 4.0)),
     'sin_emb8_joint_h128_l2': (DynamicsConfig(n_layers=2, sin_embedding=True, edge_embedding_dim=8, update_pocket_coords=True,
                                               hidden_nf=128, joint_nf=32), [10, 7], [30, 36], 30, 14, 0.045, None, (1.0, 4.0)),
+    # high degree at H=256: a fully connected 150-node graph (every receiver's edges fill more than one 128-row edge tile)
+    # next to a small one, no cut-offs
+    'fc150_h256_l2': (DynamicsConfig(n_layers=2, edge_cutoff_pocket=None, edge_cutoff_interaction=None), [50, 4], [100, 9],
+                      31, 15, 0.045, None, (1.0, 4.0)),
 }
 
 

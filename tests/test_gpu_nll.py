@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-from ddpm_cases import DDPM_CFG, JOINT_CFG, OracleDynamics, make_pocket
+from ddpm_cases import DDPM_CFG, DDPM_SHAPES, JOINT_CFG, OracleDynamics, assert_fp64_bound, ddpm_shape, make_pocket
 from nll_cases import NLL_CASES, RETURN_NAMES, ddpm_kwargs, make_case_ligand
 from diffsbdd_b200 import _native, synthetic as syn
 from diffsbdd_b200.conditional_model import ConditionalDDPM, SimpleConditionalDDPM
@@ -107,6 +107,35 @@ def test_fused_vlb_terms_match_torch(joint, vnode):
     assert torch.allclose(hat, want_hat, rtol=1e-5, atol=1e-6)
     again, hat2 = _launch(side_l, side_p, lm, pm, coef, nv, nb, vnode, A, R, n)
     assert torch.equal(again, got) and torch.equal(hat2, hat)         # fixed-order reduction: bit for bit
+
+
+@pytest.mark.parametrize('with_pocket', [False, True])
+@pytest.mark.parametrize('shape', sorted(DDPM_SHAPES))
+def test_fused_noise_kernel_matches_torch(shape, with_pocket):
+    """dsb_ddpm_noise: z = alpha[g] xh + sigma[g] eps on ligand rows and, for the joint model, pocket rows (skipped when the
+    pocket pointer is NULL), one 128-thread block per graph."""
+    g = torch.Generator().manual_seed(13 + with_pocket)
+    n_lig, n_poc = ddpm_shape(shape, [7, 1, 13], [30, 5, 11])
+    A, R, B = 10, 12, len(n_lig)
+    NL, NP = sum(n_lig), sum(n_poc)
+    lm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_lig)).cuda()
+    pm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_poc)).cuda()
+    xl, el = torch.randn((NL, 3 + A), generator=g).cuda(), torch.randn((NL, 3 + A), generator=g).cuda()
+    xp, ep = torch.randn((NP, 3 + R), generator=g).cuda(), torch.randn((NP, 3 + R), generator=g).cuda()
+    coef = (torch.rand((B, 2), generator=g) * 0.9 + 0.05).cuda()
+    zl = torch.full_like(xl, float('nan'))
+    zp = torch.full_like(xp, float('nan'))
+    lib = _native.load()
+    ptr = lambda x: x.data_ptr() if with_pocket else None
+    _native.check(lib.dsb_ddpm_noise(xl.data_ptr(), el.data_ptr(), ptr(xp), ptr(ep), coef.data_ptr(), lm.data_ptr(), pm.data_ptr(),
+                                     NL, NP, B, A, R, zl.data_ptr(), ptr(zp), C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    torch.cuda.synchronize()
+    ref = lambda x, e, m, dt: coef.to(dt)[m, 0:1] * x.to(dt) + coef.to(dt)[m, 1:2] * e.to(dt)
+    assert_fp64_bound(zl, ref(xl, el, lm, torch.float32), ref(xl, el, lm, torch.float64), f'{shape} ligand')
+    if with_pocket:
+        assert_fp64_bound(zp, ref(xp, ep, pm, torch.float32), ref(xp, ep, pm, torch.float64), f'{shape} pocket')
+    else:
+        assert torch.isnan(zp).all()                 # pocket output untouched
 
 
 # ---- native forward against the eager forward and the CPU oracle -------------------------------------------------------

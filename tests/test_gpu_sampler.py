@@ -6,7 +6,7 @@ import ctypes as C
 import pytest
 import torch
 
-from ddpm_cases import DDPM_CFG, HIST, make_pocket, make_ligand
+from ddpm_cases import DDPM_CFG, DDPM_SHAPES, HIST, assert_fp64_bound, ddpm_shape, make_pocket, make_ligand
 from oracle.cpu_denoiser import OracleDynamics
 from diffsbdd_b200 import _native, synthetic as syn
 from diffsbdd_b200.conditional_model import ConditionalDDPM
@@ -31,35 +31,52 @@ def build(T, device, native=True, engine='auto'):
 
 
 def test_fused_ddpm_update_kernel_matches_torch():
+    """dsb_ddpm_ligand_update against the torch ops of the eager reverse step, out of place and in place, at every batch
+    shape of ddpm_cases.DDPM_SHAPES (one 128-thread block per graph: up to 150 ligand and 300 pocket rows per block)."""
+    for shape in sorted(DDPM_SHAPES):
+        _check_fused_ddpm_update(shape)
+
+
+def _check_fused_ddpm_update(shape):
     g = torch.Generator().manual_seed(0)
-    n_lig, n_poc = [5, 1, 9], [11, 7, 3]
-    A, R = 10, 10
-    lm = torch.repeat_interleave(torch.arange(3), torch.tensor(n_lig)).cuda()
-    pm = torch.repeat_interleave(torch.arange(3), torch.tensor(n_poc)).cuda()
-    z = torch.randn((15, 3 + A), generator=g).cuda()
-    eps = torch.randn((15, 3 + A), generator=g).cuda()
-    noise = torch.randn((15, 3 + A), generator=g).cuda()
-    pocket = torch.randn((21, 3 + R), generator=g).cuda()
-    coef = (torch.rand((3, 3), generator=g) + 0.5).cuda()
-    mu = z / coef[lm, 0:1] - coef[lm, 1:2] * eps
-    want = mu + coef[lm, 2:3] * noise
-    com = scatter_mean(want[:, :3], lm)
-    want[:, :3] -= com[lm]
-    want_p = pocket.clone()
-    want_p[:, :3] -= com[pm]
+    n_lig, n_poc = ddpm_shape(shape, [5, 1, 9], [11, 7, 3])
+    A, R, B = 10, 10, len(n_lig)
+    NL, NP = sum(n_lig), sum(n_poc)
+    lm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_lig)).cuda()
+    pm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_poc)).cuda()
+    z = torch.randn((NL, 3 + A), generator=g).cuda()
+    eps = torch.randn((NL, 3 + A), generator=g).cuda()
+    noise = torch.randn((NL, 3 + A), generator=g).cuda()
+    pocket = torch.randn((NP, 3 + R), generator=g).cuda()
+    coef = (torch.rand((B, 3), generator=g) + 0.5).cuda()
+
+    def ref(dtype):
+        z_, eps_, noise_, pocket_, coef_ = (x.to(dtype) for x in (z, eps, noise, pocket, coef))
+        mu = z_ / coef_[lm, 0:1] - coef_[lm, 1:2] * eps_
+        want = mu + coef_[lm, 2:3] * noise_
+        com = scatter_mean(want[:, :3], lm)
+        want[:, :3] -= com[lm]
+        want_p = pocket_.clone()
+        want_p[:, :3] -= com[pm]
+        return want, want_p
+
+    want, want_p = ref(torch.float32)
+    want64, want_p64 = ref(torch.float64)
     z_out, p_out = torch.empty_like(z), torch.empty_like(pocket)
     lib = _native.load()
     _native.check(lib.dsb_ddpm_ligand_update(z.data_ptr(), eps.data_ptr(), noise.data_ptr(), coef.data_ptr(),
-                                             lm.data_ptr(), pm.data_ptr(), pocket.data_ptr(), 15, 21, 3, A, R,
+                                             lm.data_ptr(), pm.data_ptr(), pocket.data_ptr(), NL, NP, B, A, R,
                                              z_out.data_ptr(), p_out.data_ptr(),
                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
     assert torch.allclose(z_out, want, atol=2e-6, rtol=1e-6)
     assert torch.allclose(p_out, want_p, atol=2e-6, rtol=1e-6)
+    assert_fp64_bound(z_out, want, want64, f'{shape} ligand')
+    assert_fp64_bound(p_out, want_p, want_p64, f'{shape} pocket')
     # in place
     z2, p2 = z.clone(), pocket.clone()
     _native.check(lib.dsb_ddpm_ligand_update(z2.data_ptr(), eps.data_ptr(), noise.data_ptr(), coef.data_ptr(),
-                                             lm.data_ptr(), pm.data_ptr(), p2.data_ptr(), 15, 21, 3, A, R,
+                                             lm.data_ptr(), pm.data_ptr(), p2.data_ptr(), NL, NP, B, A, R,
                                              z2.data_ptr(), p2.data_ptr(),
                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)))
     torch.cuda.synchronize()
@@ -169,10 +186,16 @@ def test_graph_loop_statistics():
 
 def test_fused_inpaint_kernel_matches_torch_ops():
     """dsb_ddpm_inpaint_update against the torch ops of the eager RePaint iteration (conditional_model.py:636-666),
-    with and without the re-noising step, ragged graphs incl. a graph without fixed atoms."""
+    with and without the re-noising step, ragged graphs incl. a graph without fixed atoms, at every batch shape of
+    ddpm_cases.DDPM_SHAPES."""
+    for shape in sorted(DDPM_SHAPES):
+        _check_fused_inpaint(shape)
+
+
+def _check_fused_inpaint(shape):
     g = torch.Generator().manual_seed(1)
-    n_lig, n_poc = [6, 1, 9, 4], [11, 7, 3, 8]
-    A, R, B = 10, 10, 4
+    n_lig, n_poc = ddpm_shape(shape, [6, 1, 9, 4], [11, 7, 3, 8])
+    A, R, B = 10, 10, len(n_lig)
     lm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_lig)).cuda()
     pm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_poc)).cuda()
     NL, NP = sum(n_lig), sum(n_poc)
@@ -181,34 +204,42 @@ def test_fused_inpaint_kernel_matches_torch_ops():
     known = torch.randn((NL, 3 + A), generator=g).cuda()
     com0 = torch.randn((B, 3), generator=g).cuda()
     fixed = (torch.rand(NL, generator=g) < 0.4).float().cuda()
-    fixed[lm == 3] = 0                       # a graph with nothing fixed
+    fixed[lm == B - 1] = 0                   # a graph with nothing fixed
     fixed[0] = 1
     n1 = torch.randn((NL, 3 + A), generator=g).cuda()
     n2 = torch.randn((NL, 3 + A), generator=g).cuda()
     coef = (torch.rand((B, 4), generator=g) * 0.8 + 0.1).cuda()
     lib = _native.load()
-    for renoise in (False, True):
-        # torch ops in eager order
-        com_pocket = scatter_mean(pocket[:, :3], pm)
-        xk = known.clone()
-        xk[:, :3] = known[:, :3] + (com_pocket - com0)[lm]
-        zk = coef[lm, 0:1] * xk + coef[lm, 1:2] * n1
-        pk = pocket.clone()
+
+    def ref(dtype, renoise):
+        """The torch ops in eager order."""
+        z_unknown_, pocket_, known_, com0_, fixed_, n1_, n2_, coef_ = (
+            x.to(dtype) for x in (z_unknown, pocket, known, com0, fixed, n1, n2, coef))
+        com_pocket = scatter_mean(pocket_[:, :3], pm)
+        xk = known_.clone()
+        xk[:, :3] = known_[:, :3] + (com_pocket - com0_)[lm]
+        zk = coef_[lm, 0:1] * xk + coef_[lm, 1:2] * n1_
+        pk = pocket_.clone()
         mean = scatter_mean(zk[:, :3], lm)
         zk[:, :3] = zk[:, :3] - mean[lm]
         pk[:, :3] = pk[:, :3] - mean[pm]
-        rows = fixed.bool()
+        rows = fixed_.bool()
         cn = scatter_mean(zk[rows][:, :3], lm[rows], dim_size=B)
-        cd = scatter_mean(z_unknown[rows][:, :3], lm[rows], dim_size=B)
+        cd = scatter_mean(z_unknown_[rows][:, :3], lm[rows], dim_size=B)
         dx = cd - cn
         zk[:, :3] = zk[:, :3] + dx[lm]
         pk[:, :3] = pk[:, :3] + dx[pm]
-        want = zk * fixed[:, None] + z_unknown * (1 - fixed[:, None])
+        want = zk * fixed_[:, None] + z_unknown_ * (1 - fixed_[:, None])
         if renoise:
-            want = coef[lm, 2:3] * want + coef[lm, 3:4] * n2
+            want = coef_[lm, 2:3] * want + coef_[lm, 3:4] * n2_
             m2 = scatter_mean(want[:, :3], lm)
             want[:, :3] = want[:, :3] - m2[lm]
             pk[:, :3] = pk[:, :3] - m2[pm]
+        return want, pk
+
+    for renoise in (False, True):
+        want, pk = ref(torch.float32, renoise)
+        want64, pk64 = ref(torch.float64, renoise)
         z, p = z_unknown.clone(), pocket.clone()
         _native.check(lib.dsb_ddpm_inpaint_update(
             z.data_ptr(), p.data_ptr(), known.data_ptr(), com0.data_ptr(), fixed.data_ptr(), n1.data_ptr(),
@@ -217,6 +248,8 @@ def test_fused_inpaint_kernel_matches_torch_ops():
         torch.cuda.synchronize()
         assert torch.allclose(z, want, atol=3e-6, rtol=1e-5), float((z - want).abs().max())
         assert torch.allclose(p, pk, atol=3e-6, rtol=1e-5), float((p - pk).abs().max())
+        assert_fp64_bound(z, want, want64, f'{shape} renoise={renoise} ligand')
+        assert_fp64_bound(p, pk, pk64, f'{shape} renoise={renoise} pocket')
 
 
 @pytest.mark.parametrize('resamplings,frames', [(1, 1), (3, 2)])
@@ -370,10 +403,16 @@ def _joint_ref_noise(nx, lm, pm):
 
 def test_fused_joint_kernels_match_torch_ops():
     """dsb_ddpm_joint_update / dsb_ddpm_joint_inpaint_update against the torch ops of the eager joint sampler
-    (en_diffusion.py:503-557, :741-807), ragged graphs, partially fixed pocket, with and without the jump back."""
+    (en_diffusion.py:503-557, :741-807), ragged graphs, partially fixed pocket, with and without the jump back, at every
+    batch shape of ddpm_cases.DDPM_SHAPES."""
+    for shape in sorted(DDPM_SHAPES):
+        _check_fused_joint(shape)
+
+
+def _check_fused_joint(shape):
     g = torch.Generator().manual_seed(3)
-    n_lig, n_poc = [5, 1, 8], [9, 6, 4]
-    A, R, B = 10, 10, 3
+    n_lig, n_poc = ddpm_shape(shape, [5, 1, 8], [9, 6, 4])
+    A, R, B = 10, 10, len(n_lig)
     lm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_lig)).cuda()
     pm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_poc)).cuda()
     cm = torch.cat((lm, pm))
@@ -386,16 +425,24 @@ def test_fused_joint_kernels_match_torch_ops():
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     P = lambda t: t.data_ptr()
 
-    ex = _joint_ref_noise(nx, lm, pm)
-    eps_l, eps_p = torch.cat((ex[:NL], nhl), 1), torch.cat((ex[NL:], nhp), 1)
-    wl = zl / coef3[lm, 0:1] - coef3[lm, 1:2] * el + coef3[lm, 2:3] * eps_l
-    wp = zp / coef3[pm, 0:1] - coef3[pm, 1:2] * ep + coef3[pm, 2:3] * eps_p
-    mean = scatter_mean(torch.cat((wl[:, :3], wp[:, :3])), cm)
-    wl[:, :3] -= mean[lm]; wp[:, :3] -= mean[pm]
+    def ref_update(dtype):
+        zl_, zp_, el_, ep_, nx_, nhl_, nhp_, coef3_ = (x.to(dtype) for x in (zl, zp, el, ep, nx, nhl, nhp, coef3))
+        ex = _joint_ref_noise(nx_, lm, pm)
+        eps_l, eps_p = torch.cat((ex[:NL], nhl_), 1), torch.cat((ex[NL:], nhp_), 1)
+        wl = zl_ / coef3_[lm, 0:1] - coef3_[lm, 1:2] * el_ + coef3_[lm, 2:3] * eps_l
+        wp = zp_ / coef3_[pm, 0:1] - coef3_[pm, 1:2] * ep_ + coef3_[pm, 2:3] * eps_p
+        mean = scatter_mean(torch.cat((wl[:, :3], wp[:, :3])), cm)
+        wl[:, :3] -= mean[lm]; wp[:, :3] -= mean[pm]
+        return wl, wp
+
+    wl, wp = ref_update(torch.float32)
+    wl64, wp64 = ref_update(torch.float64)
     a, b = zl.clone(), zp.clone()
     _native.check(lib.dsb_ddpm_joint_update(P(a), P(b), P(el), P(ep), P(nx), P(nhl), P(nhp), P(coef3), P(lm), P(pm), NL, NP, B, A, R, stream))
     torch.cuda.synchronize()
     assert torch.allclose(a, wl, atol=3e-6, rtol=1e-5) and torch.allclose(b, wp, atol=3e-6, rtol=1e-5)
+    assert_fp64_bound(a, wl, wl64, f'{shape} joint update ligand')
+    assert_fp64_bound(b, wp, wp64, f'{shape} joint update pocket')
 
     x0l, x0p = rnd(NL, 3 + A), rnd(NP, 3 + R)
     fl = (torch.rand(NL, generator=g) < 0.4).float().cuda()
@@ -403,23 +450,34 @@ def test_fused_joint_kernels_match_torch_ops():
     fl[0] = 1
     coef4 = (torch.rand((B, 4), generator=g) * 0.8 + 0.1).cuda()
     n3 = (rnd(NL + NP, 3), rnd(NL, A), rnd(NP, R))
-    for jump in (False, True):
-        zkl = coef4[lm, 0:1] * x0l + coef4[lm, 1:2] * eps_l
-        zkp = coef4[pm, 0:1] * x0p + coef4[pm, 1:2] * eps_p
-        sel_l, sel_p = fl.bool(), fp.bool()
+
+    def ref_inpaint(dtype, jump):
+        zl_, zp_, nx_, nhl_, nhp_, x0l_, x0p_, fl_, fp_, coef4_ = (
+            x.to(dtype) for x in (zl, zp, nx, nhl, nhp, x0l, x0p, fl, fp, coef4))
+        ex = _joint_ref_noise(nx_, lm, pm)
+        eps_l, eps_p = torch.cat((ex[:NL], nhl_), 1), torch.cat((ex[NL:], nhp_), 1)
+        zkl = coef4_[lm, 0:1] * x0l_ + coef4_[lm, 1:2] * eps_l
+        zkp = coef4_[pm, 0:1] * x0p_ + coef4_[pm, 1:2] * eps_p
+        sel_l, sel_p = fl_.bool(), fp_.bool()
         idx = torch.cat((lm[sel_l], pm[sel_p]))
-        com_u = scatter_mean(torch.cat((zl[sel_l][:, :3], zp[sel_p][:, :3])), idx, dim_size=B)
+        com_u = scatter_mean(torch.cat((zl_[sel_l][:, :3], zp_[sel_p][:, :3])), idx, dim_size=B)
         com_k = scatter_mean(torch.cat((zkl[sel_l][:, :3], zkp[sel_p][:, :3])), idx, dim_size=B)
         shift = com_u - com_k
         zkl[:, :3] += shift[lm]; zkp[:, :3] += shift[pm]
-        wl = zkl * fl[:, None] + zl * (1 - fl[:, None])
-        wp = zkp * fp[:, None] + zp * (1 - fp[:, None])
+        wl = zkl * fl_[:, None] + zl_ * (1 - fl_[:, None])
+        wp = zkp * fp_[:, None] + zp_ * (1 - fp_[:, None])
         if jump:
-            e3 = _joint_ref_noise(n3[0], lm, pm)
-            wl = coef4[lm, 2:3] * wl + coef4[lm, 3:4] * torch.cat((e3[:NL], n3[1]), 1)
-            wp = coef4[pm, 2:3] * wp + coef4[pm, 3:4] * torch.cat((e3[NL:], n3[2]), 1)
+            n3x, n3l, n3p = (x.to(dtype) for x in n3)
+            e3 = _joint_ref_noise(n3x, lm, pm)
+            wl = coef4_[lm, 2:3] * wl + coef4_[lm, 3:4] * torch.cat((e3[:NL], n3l), 1)
+            wp = coef4_[pm, 2:3] * wp + coef4_[pm, 3:4] * torch.cat((e3[NL:], n3p), 1)
             mean = scatter_mean(torch.cat((wl[:, :3], wp[:, :3])), cm)
             wl[:, :3] -= mean[lm]; wp[:, :3] -= mean[pm]
+        return wl, wp
+
+    for jump in (False, True):
+        wl, wp = ref_inpaint(torch.float32, jump)
+        wl64, wp64 = ref_inpaint(torch.float64, jump)
         a, b = zl.clone(), zp.clone()
         j = [P(x) for x in n3] if jump else [None, None, None]
         _native.check(lib.dsb_ddpm_joint_inpaint_update(P(a), P(b), P(x0l), P(x0p), P(fl), P(fp), P(nx), P(nhl), P(nhp), *j,
@@ -427,6 +485,8 @@ def test_fused_joint_kernels_match_torch_ops():
         torch.cuda.synchronize()
         assert torch.allclose(a, wl, atol=3e-6, rtol=1e-5), float((a - wl).abs().max())
         assert torch.allclose(b, wp, atol=3e-6, rtol=1e-5), float((b - wp).abs().max())
+        assert_fp64_bound(a, wl, wl64, f'{shape} jump={jump} joint inpaint ligand')
+        assert_fp64_bound(b, wp, wp64, f'{shape} jump={jump} joint inpaint pocket')
 
 
 def _joint_pair(T):
