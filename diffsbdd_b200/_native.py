@@ -16,7 +16,7 @@ _LIB: Optional[C.CDLL] = None
 EXPORTED_SYMBOLS = (
     'dsb_param_count', 'dsb_param_name', 'dsb_dynamics_create', 'dsb_dynamics_destroy',
     'dsb_edge_capacity', 'dsb_dynamics_workspace_bytes', 'dsb_dynamics_forward', 'dsb_dynamics_edges',
-    'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
+    'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_deterministic', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
     'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_ddpm_noise',
     'dsb_ddpm_vlb_terms', 'dsb_last_error', 'dsb_version',
 )
@@ -88,6 +88,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dsb_set_programmatic_launch.restype = C.c_int
     lib.dsb_dynamics_set_math_mode.argtypes = [vp, C.c_int]
     lib.dsb_dynamics_set_math_mode.restype = C.c_int
+    lib.dsb_dynamics_set_deterministic.argtypes = [vp, C.c_int]
+    lib.dsb_dynamics_set_deterministic.restype = C.c_int
     lib.dsb_dynamics_set_profiling.argtypes = [vp, C.c_int]
     lib.dsb_dynamics_set_profiling.restype = C.c_int
     lib.dsb_dynamics_collect_profile.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(i64), C.c_int]

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 from . import _native
 from .dynamics import EGNNDynamics
-from .en_diffusion import EnVariationalDiffusion, scatter_add, scatter_mean, num_nodes_to_batch_mask
+from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_add, scatter_mean, num_nodes_to_batch_mask
 
 
 class ConditionalDDPM(EnVariationalDiffusion):
@@ -281,6 +281,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return st['z'].clone(), st['pocket'].clone()
 
     # ---- public samplers ------------------------------------------------------------------------------------
+    @follows_dynamics_determinism
     @torch.no_grad()
     def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None):
         """conditional_model.py:479-555."""
@@ -335,6 +336,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lig_mask, pocket['mask']
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def inpaint(self, ligand, pocket, lig_fixed, resamplings=1, return_frames=1, timesteps=None, center='ligand'):
         """conditional_model.py:558-686: RePaint-style conditional generation with fixed ligand atoms."""
@@ -445,6 +447,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
             z.data_ptr(), pocket_out.data_ptr(), C.c_void_p(torch.cuda.current_stream(xh_lig.device).cuda_stream)))
         return z, pocket_out
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def forward(self, ligand, pocket, return_info=False):
         """Eval-mode variational bound (conditional_model.py:202-330): the terms of -log p(x, h | N, pocket) of the ligand
@@ -515,6 +518,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
             xh0_lig[:, :self.n_dims], xh0_pocket[:, :self.n_dims], ligand['mask'], pocket['mask'])
         return self.noised_representation(xh0_lig, xh0_pocket, ligand['mask'], pocket['mask'], gamma_t)
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def diversify(self, ligand, pocket, noising_steps):
         """conditional_model.py:364-409: partially noise given ligands, then denoise them again."""
@@ -560,6 +564,7 @@ class SimpleConditionalDDPM(ConditionalDDPM):
         z_lig, _ = self._native_noise(xh_lig, eps, None, None, lig_mask, pocket_mask, gamma)   # no COM projection
         return z_lig, xh_pocket
 
+    @follows_dynamics_determinism
     def forward(self, ligand, pocket, return_info=False):
         """conditional_model.py:727-735: the likelihood is evaluated in the frame of the pocket's centre of mass."""
         pocket_com = scatter_mean(pocket['x'], pocket['mask'], dim=0)
@@ -567,6 +572,7 @@ class SimpleConditionalDDPM(ConditionalDDPM):
         pocket['x'] = pocket['x'] - pocket_com[pocket['mask']]
         return super().forward(ligand, pocket, return_info)
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None):
         pocket_com = scatter_mean(pocket['x'], pocket['mask'], dim=0)

@@ -307,7 +307,7 @@ static int pack_weights(dsb_dynamics* d, const float* const* params, const std::
 }
 
 // ---- workspace --------------------------------------------------------------------------------------------
-static Workspace carve(const dsb_config& c, int64_t NL, int64_t NP, int64_t B, int64_t Ecap, void* base) {
+static Workspace carve(const dsb_config& c, int64_t NL, int64_t NP, int64_t B, int64_t Ecap, bool det, void* base) {
   Workspace ws;
   const int64_t N = NL + NP;
   const int H = c.hidden_nf;
@@ -331,6 +331,12 @@ static Workspace carve(const dsb_config& c, int64_t NL, int64_t NP, int64_t B, i
   ws.erow = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1));
   ws.ecol = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1));
   ws.ed0 = (float*)take(sizeof(float) * (size_t)(Ecap + 1));
+  // deterministic mode: one H-wide slot per 4-row chunk of the 128-row tiles that cover the virtual edge order (the
+  // coordinate kernels use nm float4 per chunk, at most 8 floats <= H)
+  const int64_t vtiles = (Ecap + (kRowChunk - 1) * N + 127) / 128;
+  ws.part = det ? (float*)take(sizeof(float) * (size_t)(vtiles * (128 / kRowChunk)) * H) : nullptr;
+  const int64_t vrows = Ecap + (kRowChunk - 1) * N;
+  ws.vcap = (int32_t)(vrows < INT32_MAX ? vrows : INT32_MAX);
   ws.bytes = off;
   return ws;
 }
@@ -812,7 +818,7 @@ int64_t dsb_edge_capacity(const int64_t* n_lig, const int64_t* n_pocket, int n_g
 size_t dsb_dynamics_workspace_bytes(const dsb_dynamics* dyn, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
                                     int64_t edge_capacity) {
   if (!dyn || check_sizes(n_atoms, n_residues, n_graphs, edge_capacity)) return 0;
-  return carve(dyn->cfg, n_atoms, n_residues, n_graphs, edge_capacity, nullptr).bytes + 256;
+  return carve(dyn->cfg, n_atoms, n_residues, n_graphs, edge_capacity, dyn->deterministic != 0, nullptr).bytes + 256;
 }
 
 static int setup(dsb_dynamics* dyn, int64_t n_atoms, int64_t n_residues, int64_t n_graphs, int64_t edge_capacity,
@@ -821,7 +827,7 @@ static int setup(dsb_dynamics* dyn, int64_t n_atoms, int64_t n_residues, int64_t
   if (int e = check_sizes(n_atoms, n_residues, n_graphs, edge_capacity)) return e;
   if (!workspace) { set_error("null workspace"); return DSB_ERR_INVALID_ARGUMENT; }
   char* base = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  *ws = carve(dyn->cfg, n_atoms, n_residues, n_graphs, edge_capacity, base);
+  *ws = carve(dyn->cfg, n_atoms, n_residues, n_graphs, edge_capacity, dyn->deterministic != 0, base);
   if ((size_t)(base - (char*)workspace) + ws->bytes > workspace_bytes) {
     set_error("workspace too small: need %zu bytes, got %zu", ws->bytes + 256, workspace_bytes);
     return DSB_ERR_WORKSPACE_TOO_SMALL;
@@ -895,6 +901,7 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
 #define DSB_TRY(expr) do { if (int e_ = (expr)) return e_; } while (0)
   const int mm = (tc_width_supported(H) && !c.sin_embedding) ? dyn->math_mode : 0;      // sin_embedding: fp32 FFMA kernels only
   const bool f16 = (mm & 8) != 0;
+  const bool det = dyn->deterministic != 0;
   auto gemm = [&](const GemmArgs& ga, const TcImage& img, int n_tile_off = 0) -> int {
     return ((mm & 1) && img.t_hi) ? launch_tc_node_gemm(dyn, ga, img, n_tile_off, f16, status, s) : launch_node_gemm(ga, s);
   };
@@ -927,6 +934,10 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
       }
       mark(KC_EDGE_GCL);
       DSB_TRY((mm & 2) ? launch_tc_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, f16, status, s) : launch_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, s));
+      if (det) {              // fixed-order receiver sums: agg = per-receiver sums of the chunk partials (one slot per chunk)
+        DSB_TRY(launch_segment_reduce(ws, dm.N, H / 4, 1, reinterpret_cast<float4*>(ws.agg), s));
+        launches += 1;
+      }
       // node_model: h + W4 SiLU(W3 [h | agg/norm] + b3) + b4   (egnn_new.py:48-58)
       mark(KC_NODE_GEMM);
       GemmArgs g2 = {ws.h, H, H, ws.agg, H, H, c.normalization_factor, G.W3, H, G.b3, nullptr, 0, ws.hT, H, dm.N, H, 1, nullptr, 0, 0, 0,
@@ -945,6 +956,10 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
     DSB_TRY(gemm(g4, Q.iW1));
     mark(KC_EDGE_COORD);
     DSB_TRY((mm & 4) ? launch_tc_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, f16, status, s) : launch_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, s));
+    if (det && dm.n_coord_rows > 0) {   // xagg rows of the moving nodes; the tensor-core kernel keeps one slot per chunk and MLP
+      DSB_TRY(launch_segment_reduce(ws, dm.n_coord_rows, 1, (mm & 4) ? nm : 1, ws.xagg, s));
+      launches += 1;
+    }
     float4* xnext = ws.xbuf[1 + (l & 1)];
     mark(KC_COORD_FINISH);
     DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, xnext, true, s));
@@ -974,6 +989,13 @@ int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode) {
   if (mode != 0 && !tc_width_supported(dyn->cfg.hidden_nf)) { set_error("the tensor-core kernels are built for hidden_nf 128, 192 and 256 only"); return DSB_ERR_UNSUPPORTED_CONFIG; }
   dyn->math_mode = mode;
   return 0;
+}
+
+int dsb_dynamics_set_deterministic(dsb_dynamics* dyn, int enable) {
+  if (!dyn) { set_error("null handle"); return DSB_ERR_INVALID_ARGUMENT; }
+  const int old = dyn->deterministic;
+  if (enable >= 0) dyn->deterministic = enable != 0;
+  return old;
 }
 
 int dsb_dynamics_set_profiling(dsb_dynamics* dyn, int enabled) {

@@ -15,6 +15,10 @@
 //   4. epilogue in registers: +b2, SiLU, attention gate (half-warp shuffle reduce) or phi = w3 . m
 //   5. deterministic-order segmented sum over the tile's rows through shared memory; one RED per
 //      (receiver segment, column) into the zero-initialised aggregate — no per-edge atomics.
+// DET (deterministic mode): the tiles run over the padded virtual edge order of the tensor-core kernels (vrow_ptr / vmap:
+// every receiver starts at a multiple of kRowChunk rows), step 5 stores the in-order sum of every 4-row chunk into the
+// chunk's slot of Workspace::part, and launch_segment_reduce sums each receiver's chunks in ascending order.  A receiver's
+// sum then depends on its own edges only, not on where the 128-edge tiles fall or on the order the tiles finish.
 #include "dsb_internal.cuh"
 
 namespace dsb {
@@ -166,9 +170,11 @@ struct EdgeGclArgs {
   const int32_t *erow, *ecol; const float* ed0; int NL;
   GclW w;
   float* agg;                        // [N][H], zero on entry; receives raw sums
+  const int32_t* vrow_ptr; const int32_t* vmap; float* part;   // DET: virtual rows, chunk partials [chunk][H]
+  int vcap;                                                     // DET: virtual rows covered by vmap / part
 };
 
-template <int H, bool SIN>
+template <int H, bool SIN, bool DET = false>
 __global__ void __launch_bounds__(ETHREADS, 1) edge_gcl_kernel(EdgeGclArgs a) {
   extern __shared__ __align__(16) float smem[];
   using S = EdgeSmem<H>;
@@ -194,15 +200,15 @@ __global__ void __launch_bounds__(ETHREADS, 1) edge_gcl_kernel(EdgeGclArgs a) {
     if (has_tb) { s_tb[i] = a.w.tb[i]; s_tb[H + i] = a.w.tb[H + i]; s_tb[2 * H + i] = a.w.tb[2 * H + i]; }
   }
   const float ba = has_att ? a.w.ba[0] : 0.f;
-  const int E = a.row_ptr[a.N];
+  const int E = DET ? min(a.vrow_ptr[a.N], a.vcap) : a.row_ptr[a.N];
   __syncthreads();
 
 #pragma unroll 1
   for (int e0 = blockIdx.x * EBM; e0 < E; e0 += gridDim.x * EBM) {
     if (tid < EBM) {
-      const int e = e0 + tid;
+      const int e = DET ? (e0 + tid < E ? a.vmap[e0 + tid] : -1) : e0 + tid;
       int r = -1, c = 0, ty_ = 0; float d2 = 0.f, d0 = 0.f;
-      if (e < E) {
+      if (DET ? e >= 0 : e < E) {
         r = a.erow[e]; c = a.ecol[e]; d0 = a.ed0[e];
         const float4 xi = a.x[r], xj = a.x[c];
         const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
@@ -255,7 +261,20 @@ __global__ void __launch_bounds__(ETHREADS, 1) edge_gcl_kernel(EdgeGclArgs a) {
       __syncthreads();
       const int c = tid & 127, rh = tid >> 7;
       const int ncols = (H - 128 * pass) < 128 ? (H - 128 * pass) : 128;
-      if (c < ncols) {
+      if constexpr (DET) {
+        if (c < ncols) {
+          constexpr int NCH = EBM / kRowChunk;
+          for (int k = rh * (NCH / 2); k < (rh + 1) * (NCH / 2); ++k) {
+            float sum = 0.f;
+#pragma unroll
+            for (int i = 0; i < kRowChunk; ++i) {
+              const int r = k * kRowChunk + i;
+              if (s_row[r] >= 0) sum += Es[r * 132 + c];
+            }
+            a.part[(size_t)(e0 / kRowChunk + k) * H + 128 * pass + c] = sum;
+          }
+        }
+      } else if (c < ncols) {
         int cur = -1; float sum = 0.f;
         for (int r = rh * 64; r < rh * 64 + 64; ++r) {
           const int row = s_row[r];
@@ -281,9 +300,11 @@ struct EdgeCoordArgs {
   EquivW w; int nm;                  // nm = 1 (reflection equivariant) or 2 (+ cross-product MLP)
   float norm_constant, coords_range; int use_tanh;
   float4* xagg;                      // [N], zero on entry; receives raw sums of trans
+  const int32_t* vrow_ptr; const int32_t* vmap; float4* part;  // DET: virtual rows, chunk partials [chunk] (both MLPs summed)
+  int vcap;                                                     // DET: virtual rows covered by vmap / part
 };
 
-template <int H, bool SIN>
+template <int H, bool SIN, bool DET = false>
 __global__ void __launch_bounds__(ETHREADS, 1) edge_coord_kernel(EdgeCoordArgs a) {
   extern __shared__ __align__(16) float smem[];
   using S = EdgeSmem<H>;
@@ -310,16 +331,16 @@ __global__ void __launch_bounds__(ETHREADS, 1) edge_coord_kernel(EdgeCoordArgs a
     }
     s_w3[i] = a.w.w3[i];
   }
-  const int E = a.row_ptr[a.n_rows];
+  const int E = DET ? min(a.vrow_ptr[a.n_rows], a.vcap) : a.row_ptr[a.n_rows];
   __syncthreads();
 
 #pragma unroll 1
   for (int e0 = blockIdx.x * EBM; e0 < E; e0 += gridDim.x * EBM) {
     if (tid < EBM) {
-      const int e = e0 + tid;
+      const int e = DET ? (e0 + tid < E ? a.vmap[e0 + tid] : -1) : e0 + tid;
       int r = -1, c = 0, ty_ = 0; float d2 = 0.f, d0 = 0.f;
       float dir[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (e < E) {
+      if (DET ? e >= 0 : e < E) {
         r = a.erow[e]; c = a.ecol[e]; d0 = a.ed0[e];
         const float4 xi = a.x[r], xj = a.x[c];
         const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
@@ -383,7 +404,17 @@ __global__ void __launch_bounds__(ETHREADS, 1) edge_coord_kernel(EdgeCoordArgs a
       }
     }
     __syncthreads();
-    if (tid < 3) {      // in-order segmented sum (egnn_new.py:114-116)
+    if constexpr (DET) {
+      if (tid < EBM / kRowChunk) {      // in-order 4-row chunk sums -> the chunk's slot
+        float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+        for (int i = 0; i < kRowChunk; ++i) {
+          const int r = tid * kRowChunk + i;
+          if (s_row[r] >= 0) { sum.x += s_tr[r]; sum.y += s_tr[EBM + r]; sum.z += s_tr[2 * EBM + r]; }
+        }
+        a.part[e0 / kRowChunk + tid] = sum;
+      }
+    } else if (tid < 3) {      // in-order segmented sum (egnn_new.py:114-116)
       int cur = -1; float sum = 0.f;
       float* dst = reinterpret_cast<float*>(a.xagg);
       for (int r = 0; r < EBM; ++r) {
@@ -408,12 +439,27 @@ template <int H> static size_t coord_smem_bytes() {
   return sizeof(float) * (size_t)(EdgeSmem<H>::kMainAlloc + 13 * H + 10 * EBM) + sizeof(int) * 3 * EBM;
 }
 
-template <int H> static int configure_h() {
-  DSB_CUDA_OK(cudaFuncSetAttribute(edge_gcl_kernel<H, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gcl_smem_bytes<H>()));
-  DSB_CUDA_OK(cudaFuncSetAttribute(edge_coord_kernel<H, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coord_smem_bytes<H>()));
-  DSB_CUDA_OK(cudaFuncSetAttribute(edge_gcl_kernel<H, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gcl_smem_bytes<H>()));
-  DSB_CUDA_OK(cudaFuncSetAttribute(edge_coord_kernel<H, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coord_smem_bytes<H>()));
+template <int H, bool DET> static int configure_variant() {
+  DSB_CUDA_OK(cudaFuncSetAttribute(edge_gcl_kernel<H, false, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gcl_smem_bytes<H>()));
+  DSB_CUDA_OK(cudaFuncSetAttribute(edge_coord_kernel<H, false, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coord_smem_bytes<H>()));
+  DSB_CUDA_OK(cudaFuncSetAttribute(edge_gcl_kernel<H, true, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gcl_smem_bytes<H>()));
+  DSB_CUDA_OK(cudaFuncSetAttribute(edge_coord_kernel<H, true, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)coord_smem_bytes<H>()));
   return 0;
+}
+template <int H> static int configure_h() {
+  if (int e = configure_variant<H, false>()) return e;
+  return configure_variant<H, true>();
+}
+
+template <int H> static void run_gcl(const EdgeGclArgs& a, bool sin, bool det, int grid, cudaStream_t s) {
+  const size_t sm = gcl_smem_bytes<H>();
+  if (det) { if (sin) edge_gcl_kernel<H, true, true><<<grid, ETHREADS, sm, s>>>(a); else edge_gcl_kernel<H, false, true><<<grid, ETHREADS, sm, s>>>(a); }
+  else { if (sin) edge_gcl_kernel<H, true><<<grid, ETHREADS, sm, s>>>(a); else edge_gcl_kernel<H, false><<<grid, ETHREADS, sm, s>>>(a); }
+}
+template <int H> static void run_coord(const EdgeCoordArgs& a, bool sin, bool det, int grid, cudaStream_t s) {
+  const size_t sm = coord_smem_bytes<H>();
+  if (det) { if (sin) edge_coord_kernel<H, true, true><<<grid, ETHREADS, sm, s>>>(a); else edge_coord_kernel<H, false, true><<<grid, ETHREADS, sm, s>>>(a); }
+  else { if (sin) edge_coord_kernel<H, true><<<grid, ETHREADS, sm, s>>>(a); else edge_coord_kernel<H, false><<<grid, ETHREADS, sm, s>>>(a); }
 }
 
 int configure_edge_kernels(int H) {
@@ -432,13 +478,14 @@ int launch_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, 
   EdgeGclArgs a;
   a.P = pv.P; a.ldp = pv.ldp; a.x = x; a.row_ptr = ws.row_ptr; a.N = dm.N;
   a.erow = ws.erow; a.ecol = ws.ecol; a.ed0 = ws.ed0; a.NL = dm.NL; a.w = w; a.agg = ws.agg;
+  a.vrow_ptr = ws.vrow_ptr; a.vmap = ws.vmap; a.part = ws.part; a.vcap = ws.vcap;
   const int grid = d->num_sms;
-  const bool sin = d->cfg.sin_embedding != 0;
+  const bool sin = d->cfg.sin_embedding != 0, det = d->deterministic != 0;
   switch (H) {
-    case 64: if (sin) edge_gcl_kernel<64, true><<<grid, ETHREADS, gcl_smem_bytes<64>(), s>>>(a); else edge_gcl_kernel<64, false><<<grid, ETHREADS, gcl_smem_bytes<64>(), s>>>(a); break;
-    case 128: if (sin) edge_gcl_kernel<128, true><<<grid, ETHREADS, gcl_smem_bytes<128>(), s>>>(a); else edge_gcl_kernel<128, false><<<grid, ETHREADS, gcl_smem_bytes<128>(), s>>>(a); break;
-    case 192: if (sin) edge_gcl_kernel<192, true><<<grid, ETHREADS, gcl_smem_bytes<192>(), s>>>(a); else edge_gcl_kernel<192, false><<<grid, ETHREADS, gcl_smem_bytes<192>(), s>>>(a); break;
-    case 256: if (sin) edge_gcl_kernel<256, true><<<grid, ETHREADS, gcl_smem_bytes<256>(), s>>>(a); else edge_gcl_kernel<256, false><<<grid, ETHREADS, gcl_smem_bytes<256>(), s>>>(a); break;
+    case 64: run_gcl<64>(a, sin, det, grid, s); break;
+    case 128: run_gcl<128>(a, sin, det, grid, s); break;
+    case 192: run_gcl<192>(a, sin, det, grid, s); break;
+    case 256: run_gcl<256>(a, sin, det, grid, s); break;
     default: return DSB_ERR_UNSUPPORTED_CONFIG;
   }
   DSB_CUDA_OK(cudaGetLastError());
@@ -456,16 +503,46 @@ int launch_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws
   a.erow = ws.erow; a.ecol = ws.ecol; a.ed0 = ws.ed0; a.NL = dm.NL; a.w = w;
   a.norm_constant = c.norm_constant; a.coords_range = c.coords_range; a.use_tanh = c.tanh;
   a.xagg = ws.xagg;
+  a.vrow_ptr = ws.vrow_ptr; a.vmap = ws.vmap; a.part = reinterpret_cast<float4*>(ws.part); a.vcap = ws.vcap;
   const int grid = d->num_sms;
-  const bool sin = c.sin_embedding != 0;
+  const bool sin = c.sin_embedding != 0, det = d->deterministic != 0;
   switch (H) {
-    case 64: if (sin) edge_coord_kernel<64, true><<<grid, ETHREADS, coord_smem_bytes<64>(), s>>>(a); else edge_coord_kernel<64, false><<<grid, ETHREADS, coord_smem_bytes<64>(), s>>>(a); break;
-    case 128: if (sin) edge_coord_kernel<128, true><<<grid, ETHREADS, coord_smem_bytes<128>(), s>>>(a); else edge_coord_kernel<128, false><<<grid, ETHREADS, coord_smem_bytes<128>(), s>>>(a); break;
-    case 192: if (sin) edge_coord_kernel<192, true><<<grid, ETHREADS, coord_smem_bytes<192>(), s>>>(a); else edge_coord_kernel<192, false><<<grid, ETHREADS, coord_smem_bytes<192>(), s>>>(a); break;
-    case 256: if (sin) edge_coord_kernel<256, true><<<grid, ETHREADS, coord_smem_bytes<256>(), s>>>(a); else edge_coord_kernel<256, false><<<grid, ETHREADS, coord_smem_bytes<256>(), s>>>(a); break;
+    case 64: run_coord<64>(a, sin, det, grid, s); break;
+    case 128: run_coord<128>(a, sin, det, grid, s); break;
+    case 192: run_coord<192>(a, sin, det, grid, s); break;
+    case 256: run_coord<256>(a, sin, det, grid, s); break;
     default: return DSB_ERR_UNSUPPORTED_CONFIG;
   }
   DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// =====================================================================================================
+// deterministic mode: fixed-order receiver sums from the chunk partials of the edge kernels.  One thread per (receiver,
+// float4 column group); it adds the receiver's slots one after another in ascending order, so the result is a function of
+// the slot contents alone (no atomics, no dependence on the grid).
+__global__ void __launch_bounds__(256) segment_reduce_kernel(const float4* __restrict__ part, int ld4,
+                                                             const int32_t* __restrict__ vrow_ptr, int vcap, int n_rows,
+                                                             int spc, float4* __restrict__ out) {
+  pdl_trigger();
+  pdl_wait();
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)n_rows * ld4) return;
+  const int i = (int)(idx / ld4), c = (int)(idx - (int64_t)i * ld4);
+  const int k0 = (min(vrow_ptr[i], vcap) / kRowChunk) * spc, k1 = (min(vrow_ptr[i + 1], vcap) / kRowChunk) * spc;
+  float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = k0; k < k1; ++k) {
+    const float4 v = part[(size_t)k * ld4 + c];
+    sum.x += v.x; sum.y += v.y; sum.z += v.z; sum.w += v.w;
+  }
+  out[(size_t)i * ld4 + c] = sum;
+}
+
+int launch_segment_reduce(const Workspace& ws, int n_rows, int ld4, int spc, float4* out, cudaStream_t s) {
+  if (n_rows == 0) return 0;
+  const int64_t tot = (int64_t)n_rows * ld4;
+  DSB_CUDA_OK(launch_k(segment_reduce_kernel, (unsigned)((tot + 255) / 256), 256, 0, s,
+                       reinterpret_cast<const float4*>(ws.part), ld4, (const int32_t*)ws.vrow_ptr, (int)ws.vcap, n_rows, spc, out));
   return 0;
 }
 

@@ -89,6 +89,10 @@ struct Workspace {
   int32_t *vrow_ptr, *vmap;     // [N+1], [Ecap + 3N]: receiver segments padded to multiples of kRowChunk rows (tensor-core edge kernels)
   int32_t *erow, *ecol;         // [Ecap]
   float *ed0;                   // [Ecap]
+  float *part;                  // deterministic mode only (else nullptr): per-chunk partial sums of the receiver reductions,
+                                //   [virtual 4-row chunk (x MLP unit)][H] for agg, [chunk (x MLP unit)] float4 for xagg
+  int32_t vcap;                 // virtual rows vmap and part cover (edge_capacity + 3N, clamped to int range): the
+                                //   deterministic kernels stop there if the edges overflowed edge_capacity (status[2])
   size_t bytes;
 };
 
@@ -114,6 +118,7 @@ struct dsb_dynamics {
   size_t blob_floats = 0;
   int num_sms = 132;
   int math_mode = 0;         // bitmask: 1 node GEMMs, 2 edge_gcl, 4 edge_coord on wgmma (H in {128,192,256}); 8: 3xFP16 split instead of 3xTF32
+  int deterministic = 0;     // 1: fixed-order receiver sums (chunk partials + segment reduce) instead of atomics
   int last_launches = 0;     // kernels only
   int last_memsets = 0;
   // profiling
@@ -196,6 +201,9 @@ int launch_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, 
 int launch_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w,
                       const float4* x, PView pv, cudaStream_t s);
 int configure_edge_kernels(int H);
+// deterministic mode: out[i] = sum of receiver i's partial slots [spc * vrow_ptr[i] / kRowChunk, spc * vrow_ptr[i+1] / kRowChunk)
+// in ascending order (ld4 float4 per slot and per output row), plain stores; rows without edges get 0
+int launch_segment_reduce(const Workspace& ws, int n_rows, int ld4, int spc, float4* out, cudaStream_t s);
 
 // ---- tensor-core path (dsb_tc.cu) --------------------------------------------------------------------
 void launch_pack_b_image(float* hi, float* lo, const float* src, int lds, int scol, int n_rows, int n_dst_off, int K, int tn);

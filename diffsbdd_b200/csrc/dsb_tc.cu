@@ -248,6 +248,8 @@ struct TcEdgeArgs {
   float* agg;                                // GCL: [N][H] raw sums
   float4* xagg;                              // coord: [N] raw sums of trans
   float inv_scale[2];                        // 3xFP16: 1 / (X_SCALE * W2 scale) per MLP; 1 for 3xTF32
+  float* part;                               // deterministic variant: chunk partials (Workspace::part) instead of agg / xagg
+  int vcap;                                  // deterministic variant: virtual rows covered by vmap / part (Workspace::vcap)
 };
 
 // per-edge scalars of edge tile v0/TM for MLP m (thread pr handles virtual row v0 + pr)
@@ -295,7 +297,10 @@ __device__ __forceinline__ void edge_scalars(const TcEdgeArgs& a, EdgeExtra<H>* 
 //          kRowChunk = 4 virtual rows, so the 4 rows of a chunk (lanes 4 and 8 apart) are summed by shuffles and one lane
 //          per chunk and column pair issues a vector RED;
 //   coord: xagg[recv] += dir * f(s) (egnn_new.py:100-109), chunk sums by shuffles, one atomic per chunk and component.
-template <bool COORD, bool F16, int H, bool TB>
+// DET (deterministic mode): the same chunk sums are stored, not added, into slot (virtual chunk) of a.part (coord: slot
+// chunk * nm + m, one float4); launch_segment_reduce then sums each receiver's slots in ascending order.  The chunk sums
+// have a fixed content and order, so the receiver sums depend on the receiver's own edges only.
+template <bool COORD, bool F16, int H, bool TB, bool DET = false>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
   using G = Geo<H>;
   constexpr int HPC = F16 ? 2 : 1;             // 32-k halves per pipeline chunk
@@ -318,7 +323,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
   if (threadIdx.x == 0) control_init(ctl);
   __syncthreads();
   pdl_wait();                 // everything above touches only kernel arguments and constant weights
-  const int E = a.vrow_ptr[a.n_rows];          // virtual rows: every receiver's edges start at a multiple of kRowChunk
+  // virtual rows: every receiver's edges start at a multiple of kRowChunk (DET: never past the partial buffer)
+  const int E = DET ? min(a.vrow_ptr[a.n_rows], a.vcap) : a.vrow_ptr[a.n_rows];
   const int n_units = ((E + TM - 1) / TM) * nm;
   const int n_my = ((int)blockIdx.x < n_units) ? (n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
   if (n_my == 0) return;
@@ -436,8 +442,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
       float g_lo = has_att ? sigmoid_f(s_lo + ba) : 1.0f, g_hi = has_att ? sigmoid_f(s_hi + ba) : 1.0f;
       g_lo = row_lo >= 0 ? g_lo : 0.f;
       g_hi = row_hi >= 0 ? g_hi : 0.f;
-      float* const dst_lo = a.agg + (size_t)max(crow_lo, 0) * H + 2 * (lane & 3);
-      float* const dst_hi = a.agg + (size_t)max(crow_hi, 0) * H + 2 * (lane & 3);
+      float* const dst_lo = DET ? a.part + (size_t)((e0 + (re & ~3)) / kRowChunk) * H + 2 * (lane & 3)
+                                : a.agg + (size_t)max(crow_lo, 0) * H + 2 * (lane & 3);
+      float* const dst_hi = DET ? a.part + (size_t)((e0 + ((re + 8) & ~3)) / kRowChunk) * H + 2 * (lane & 3)
+                                : a.agg + (size_t)max(crow_hi, 0) * H + 2 * (lane & 3);
 #pragma unroll
       for (int jj = 0; jj < H / 8; ++jj) {
         float v0 = g_lo * acc[4 * jj], v1 = g_lo * acc[4 * jj + 1], v2 = g_hi * acc[4 * jj + 2], v3 = g_hi * acc[4 * jj + 3];
@@ -446,11 +454,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
         v0 += __shfl_xor_sync(0xffffffffu, v0, 8); v1 += __shfl_xor_sync(0xffffffffu, v1, 8);
         v2 += __shfl_xor_sync(0xffffffffu, v2, 8); v3 += __shfl_xor_sync(0xffffffffu, v3, 8);
         // one lane per chunk (predicated, not a branch); a chunk of padding only has gate 0 on all rows: its sums are exactly
-        // 0 and go to row 0
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
-                     "@p red.global.add.v2.f32 [%0], {%1, %2};\n\t"
-                     "@p red.global.add.v2.f32 [%3], {%4, %6};\n\t}"
-                     ::"l"(dst_lo + 8 * jj), "f"(v0), "f"(v1), "l"(dst_hi + 8 * jj), "f"(v2), "r"((int)chunk_lane), "f"(v3) : "memory");
+        // 0 and go to row 0 (DET: to the pad chunk's own slot, which no receiver reads)
+        if constexpr (DET)
+          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
+                       "@p st.global.v2.f32 [%0], {%1, %2};\n\t"
+                       "@p st.global.v2.f32 [%3], {%4, %6};\n\t}"
+                       ::"l"(dst_lo + 8 * jj), "f"(v0), "f"(v1), "l"(dst_hi + 8 * jj), "f"(v2), "r"((int)chunk_lane), "f"(v3) : "memory");
+        else
+          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
+                       "@p red.global.add.v2.f32 [%0], {%1, %2};\n\t"
+                       "@p red.global.add.v2.f32 [%3], {%4, %6};\n\t}"
+                       ::"l"(dst_lo + 8 * jj), "f"(v0), "f"(v1), "l"(dst_hi + 8 * jj), "f"(v2), "r"((int)chunk_lane), "f"(v3) : "memory");
       }
     } else {
       // ---- coord: this unit's term of trans for rows re, re + 8 (egnn_new.py:100-109), chunk sums
@@ -472,7 +486,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
           tr[k] = t;
         }
         const int crow = hh ? crow_hi : crow_lo;
-        if (chunk_lane && (lane & 3) == 0 && crow >= 0) {
+        if constexpr (DET) {
+          if (chunk_lane && (lane & 3) == 0)
+            reinterpret_cast<float4*>(a.part)[(size_t)((e0 + (r & ~3)) / kRowChunk) * nm + m] = make_float4(tr[0], tr[1], tr[2], 0.f);
+        } else if (chunk_lane && (lane & 3) == 0 && crow >= 0) {
 #pragma unroll
           for (int k = 0; k < 3; ++k) atomicAdd(reinterpret_cast<float*>(a.xagg) + (size_t)crow * 4 + k, tr[k]);
         }
@@ -516,6 +533,14 @@ int configure_tc_kernels(int H) {
     DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
     DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
     DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
     return 0;
   });
 }
@@ -556,10 +581,14 @@ int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& w
   a.W2hi[0] = f16 ? w.iW2.h_hi : w.iW2.t_hi; a.W2lo[0] = f16 ? w.iW2.h_lo : w.iW2.t_lo;
   a.inv_scale[0] = f16 ? w.iW2.h_inv : 1.0f; a.inv_scale[1] = 1.0f;
   a.wr[0] = w.wr; a.wr0[0] = w.wr0; a.tb[0] = w.tb; a.b2[0] = w.b2;
-  a.wa = w.wa; a.ba = w.ba; a.agg = ws.agg;
+  a.wa = w.wa; a.ba = w.ba; a.agg = ws.agg; a.part = ws.part; a.vcap = ws.vcap;
+  const bool det = d->deterministic != 0;
   return dispatch_width(d->cfg.hidden_nf, [&]<int W>() -> int {
     auto kern = w.tb ? (f16 ? tc_edge_kernel<false, true, W, true> : tc_edge_kernel<false, false, W, true>)
                      : (f16 ? tc_edge_kernel<false, true, W, false> : tc_edge_kernel<false, false, W, false>);
+    if (det)
+      kern = w.tb ? (f16 ? tc_edge_kernel<false, true, W, true, true> : tc_edge_kernel<false, false, W, true, true>)
+                  : (f16 ? tc_edge_kernel<false, true, W, false, true> : tc_edge_kernel<false, false, W, false, true>);
     DSB_CUDA_OK(launch_k(kern, d->num_sms, TC_THREADS, edge_smem_bytes<W>(), s, a));
     return 0;
   });
@@ -580,10 +609,14 @@ int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace&
     a.wr[m] = w.wr[m]; a.wr0[m] = w.wr0[m]; a.tb[m] = w.tb[m]; a.b2[m] = w.b2[m];
   }
   a.wa = w.w3; a.ba = nullptr;
-  a.norm_constant = c.norm_constant; a.coords_range = c.coords_range; a.use_tanh = c.tanh; a.xagg = ws.xagg;
+  a.norm_constant = c.norm_constant; a.coords_range = c.coords_range; a.use_tanh = c.tanh; a.xagg = ws.xagg; a.part = ws.part; a.vcap = ws.vcap;
+  const bool det = d->deterministic != 0;
   return dispatch_width(c.hidden_nf, [&]<int W>() -> int {
     auto kern = w.tb[0] ? (f16 ? tc_edge_kernel<true, true, W, true> : tc_edge_kernel<true, false, W, true>)
                         : (f16 ? tc_edge_kernel<true, true, W, false> : tc_edge_kernel<true, false, W, false>);
+    if (det)
+      kern = w.tb[0] ? (f16 ? tc_edge_kernel<true, true, W, true, true> : tc_edge_kernel<true, false, W, true, true>)
+                     : (f16 ? tc_edge_kernel<true, true, W, false, true> : tc_edge_kernel<true, false, W, false, true>);
     DSB_CUDA_OK(launch_k(kern, d->num_sms, TC_THREADS, edge_smem_bytes<W>(), s, a));
     return 0;
   });

@@ -27,6 +27,20 @@ from .config import DynamicsConfig
 from .synthetic import state_dict_spec
 
 
+def _parse_deterministic(value):
+    if value in (True, False, 'auto'):
+        return value
+    if isinstance(value, str):
+        v = value.strip().lower()
+        if v in ('1', 'true', 'on', 'yes'):
+            return True
+        if v in ('0', 'false', 'off', 'no'):
+            return False
+        if v in ('', 'auto'):
+            return 'auto'
+    raise ValueError(f"deterministic must be True, False or 'auto' (DSB_DETERMINISTIC: 1, 0 or auto), got {value!r}")
+
+
 class _Tree(nn.Module):
     """Parameter container that reproduces nested reference key names (e.g. ``edge_mlp.0.weight``)."""
 
@@ -153,6 +167,9 @@ class EGNNDynamics(nn.Module):
         # instead of 3xTF32; 0 = fp32 FFMA kernels.  Names: 'fp32' (0), '3xtf32' (7), '3xfp16' (15).
         # 'auto' = '3xfp16' when hidden_nf is 128, 192 or 256 (the widths with tensor-core kernels), else 'fp32'.
         self._math_mode = os.environ.get('DSB_MATH_MODE', 'auto')
+        # fixed-order receiver sums (bit-identical repeat of a call, see include/diffsbdd_b200.h): True | False | 'auto'
+        # ('auto' follows torch.are_deterministic_algorithms_enabled() at call time)
+        self._deterministic = _parse_deterministic(os.environ.get('DSB_DETERMINISTIC', 'auto'))
         self.to(device)
 
     # ---- native handle management ---------------------------------------------------------------------
@@ -191,6 +208,24 @@ class EGNNDynamics(nn.Module):
         self._math_mode = value
         if self._handle is not None:
             _native.check(_native.load().dsb_dynamics_set_math_mode(C.c_void_p(self._handle), self.math_mode))
+
+    @property
+    def deterministic(self):
+        """Deterministic mode setting: ``'auto'`` (default: follows ``torch.are_deterministic_algorithms_enabled()`` at
+        call time), ``True`` or ``False``.  Initial value from the environment variable ``DSB_DETERMINISTIC``
+        (``1``/``0``/``auto``).  When active, one forward gives bit-identical outputs for bit-identical inputs, weights and
+        math mode (same GPU model and library build), and the DDPM wrappers' per-graph sums avoid unordered atomics."""
+        return self._deterministic
+
+    @deterministic.setter
+    def deterministic(self, value):
+        self._deterministic = _parse_deterministic(value)
+
+    @property
+    def deterministic_active(self) -> bool:
+        """The effective mode of the next forward (``'auto'`` resolved against torch's deterministic switch)."""
+        d = self._deterministic
+        return torch.are_deterministic_algorithms_enabled() if d == 'auto' else bool(d)
 
     def _params_by_key(self) -> Dict[str, torch.Tensor]:
         return dict(self.named_parameters(remove_duplicate=False))
@@ -247,7 +282,7 @@ class EGNNDynamics(nn.Module):
         ws = self._workspace.data_ptr() if self._workspace is not None else 0
         stt = self._status.data_ptr() if self._status is not None else 0
         pdl = int(_native.load().dsb_set_programmatic_launch(-1))
-        return (self._handle_gen, self._handle, self.math_mode, ws, stt, pdl)
+        return (self._handle_gen, self._handle, self.math_mode, ws, stt, pdl, self.deterministic_active)
 
     def _scratch(self, device, n_atoms, n_res, n_graphs, ecap) -> torch.Tensor:
         lib = _native.load()
@@ -324,6 +359,9 @@ class EGNNDynamics(nn.Module):
         if mask_atoms.dtype != torch.int64 or mask_residues.dtype != torch.int64:
             raise RuntimeError('masks must be int64 (reference constants.py:9)')
         self._ensure_handle(device)
+        rc = _native.load().dsb_dynamics_set_deterministic(C.c_void_p(self._handle), int(self.deterministic_active))
+        if rc < 0:
+            _native.check(rc)
         n_graphs, ecap = self._plan.get(mask_atoms, mask_residues, n_graphs_hint)
         ws = self._scratch(device, xh_atoms.shape[0], xh_residues.shape[0], n_graphs, ecap)
         return device, n_graphs, ecap, ws

@@ -13,7 +13,10 @@ dispatch (lightning_modules.py:814, :837) and Lightning checkpoints (keys ``ddpm
 """
 from __future__ import annotations
 
+import contextlib
+import functools
 import math
+import threading
 from typing import Dict
 
 import numpy as np
@@ -24,15 +27,56 @@ from torch import nn
 
 # ---- torch-scatter stand-ins (README.md:60 pins torch-scatter 2.0.9; semantics: output length
 # index.max()+1 unless dim_size, mean = sum / count.clamp(min=1)) ------------------------------------
+# On CUDA, index_add_ accumulates with floating-point atomics in a timing-dependent order.  Inside
+# deterministic_reductions(True) — entered by the DDPM wrappers when their dynamics runs in deterministic mode — a CUDA
+# scatter is a segment reduction with a fixed summation order instead: rows are put in index order by a stable sort (a
+# no-op permutation for a batch mask, which is non-decreasing; the joint model also scatters two concatenated masks).
+# CPU tensors always take the index_add_ path.
+_REDUCTIONS = threading.local()
+
+
+@contextlib.contextmanager
+def deterministic_reductions(enabled=True):
+    prev = getattr(_REDUCTIONS, 'deterministic', False)
+    _REDUCTIONS.deterministic = bool(enabled)
+    try:
+        yield
+    finally:
+        _REDUCTIONS.deterministic = prev
+
+
+def follows_dynamics_determinism(fn):
+    """Runs a DDPM method inside deterministic_reductions(dynamics.deterministic_active)."""
+    @functools.wraps(fn)
+    def wrapper(self, *args, **kwargs):
+        dyn = getattr(self, 'dynamics', None)
+        if dyn is None:
+            dyn = getattr(getattr(self, 'ddpm', None), 'dynamics', None)
+        with deterministic_reductions(bool(getattr(dyn, 'deterministic_active', False))):
+            return fn(self, *args, **kwargs)
+    return wrapper
+
+
+def _ordered_segments(src, index):
+    return src.is_cuda and getattr(_REDUCTIONS, 'deterministic', False)
+
+
 def scatter_add(src, index, dim=0, dim_size=None):
     assert dim == 0
     n = (int(index.max()) + 1 if index.numel() else 0) if dim_size is None else dim_size
+    if _ordered_segments(src, index):
+        order = torch.argsort(index, stable=True)
+        lengths = torch.bincount(index, minlength=n)[:n]
+        return torch.segment_reduce(src[order], 'sum', lengths=lengths, axis=0, unsafe=True)
     out = torch.zeros((n,) + tuple(src.shape[1:]), dtype=src.dtype, device=src.device)
     return out.index_add_(0, index, src)
 
 
 def scatter_mean(src, index, dim=0, dim_size=None):
     tot = scatter_add(src, index, dim, dim_size)
+    if _ordered_segments(src, index):
+        cnt = torch.bincount(index, minlength=tot.shape[0])[:tot.shape[0]].to(src.dtype)
+        return tot / cnt.clamp(min=1).view((-1,) + (1,) * (tot.dim() - 1))
     cnt = torch.zeros(tot.shape[0], dtype=src.dtype, device=src.device)
     cnt.index_add_(0, index, torch.ones(index.shape[0], dtype=src.dtype, device=src.device))
     return tot / cnt.clamp(min=1).view((-1,) + (1,) * (tot.dim() - 1))
@@ -474,6 +518,7 @@ class EnVariationalDiffusion(nn.Module):
         st['sig'] = sig
         return g
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu'):
         """en_diffusion.py:581-651: unconditional joint sampling of ligand and pocket."""
@@ -546,6 +591,7 @@ class EnVariationalDiffusion(nn.Module):
         return scatter_mean(torch.cat((x_lig[lig_sel], x_pocket[pocket_sel])),
                             torch.cat((lig_mask[lig_sel], pocket_mask[pocket_sel])), dim=0)
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings=1, jump_length=1, return_frames=1,
                 timesteps=None):
@@ -790,6 +836,7 @@ class EnVariationalDiffusion(nn.Module):
             torch.cuda.current_stream(device).cuda_stream))
         return terms, xh_lig_hat
 
+    @follows_dynamics_determinism
     @torch.no_grad()
     def forward(self, ligand, pocket, return_info=False):
         """Eval-mode variational bound of the joint model (en_diffusion.py:336-469): the terms of -log p(x, h | N) for

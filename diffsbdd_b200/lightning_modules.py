@@ -24,7 +24,7 @@ import torch.nn.functional as F
 
 from .conditional_model import ConditionalDDPM, SimpleConditionalDDPM
 from .dynamics import EGNNDynamics
-from .en_diffusion import EnVariationalDiffusion, scatter_mean, num_nodes_to_batch_mask
+from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_mean, num_nodes_to_batch_mask
 
 try:  # pragma: no cover - not installed in the offline image
     import pytorch_lightning as pl
@@ -168,6 +168,7 @@ class LigandPocketDDPM(_Base):
         return self.prepare_pocket_from_arrays(coords, types, repeats)
 
     # ---- generation (lightning_modules.py:754-872) -------------------------------------------------------------
+    @follows_dynamics_determinism
     @torch.no_grad()
     def generate_ligand_tensors(self, pocket, num_nodes_lig=None, timesteps=None, n_nodes_bias=0, n_nodes_min=0,
                                 **kwargs):

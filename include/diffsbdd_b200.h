@@ -140,6 +140,27 @@ int dsb_set_programmatic_launch(int enable);
  * status[0]).  0 = fp32 FFMA kernels everywhere.  Only hidden_nf 128, 192 and 256 have tensor-core kernels. */
 int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode);
 
+/* ---- deterministic mode (per module; default off).  enable: 1 on, 0 off, negative = query only.  Returns the previous
+ * setting (0 or 1), or DSB_ERR_INVALID_ARGUMENT for a NULL module.
+ * Off: every receiver sum of the edge kernels (GCL aggregate, coordinate update) is accumulated with floating-point
+ * atomics, whose order depends on timing; a receiver with more than two such contributions can differ in its last bits
+ * from run to run.
+ * On: the edge kernels store per-chunk partial sums (4 rows of one receiver in the padded edge order, in row order) and
+ * one extra kernel per edge launch sums each receiver's chunks in ascending order.  The summation order of every
+ * receiver's sum is then a function of that receiver's own edges, so dsb_dynamics_forward gives bit-identical outputs
+ * for bit-identical inputs (the whole batch: every graph, in the same order), weights and math mode on the same GPU
+ * model with the same library build, independent of the run or process, eager launch vs. CUDA-graph replay,
+ * programmatic dependent launch, workspace / output addresses and the persistent grid size.  A graph's outputs do not
+ * depend bitwise on the other graphs of the batch only in math mode 0 (fp32 FFMA kernels); with any tensor-core kernel
+ * (math mode != 0) the same graph denoised alone and inside another batch can differ in the last bits (measured up to
+ * ~2e-6), so regenerating one graph bit for bit needs the same batch layout as well.  Results are not bit-identical
+ * across math modes, nor with the default mode.  If the edges of a call exceed edge_capacity (status[2]) the outputs are
+ * invalid as in the default mode; the deterministic kernels then stop at the end of the partial buffer.  Cost: dsb_dynamics_workspace_bytes grows by a partial buffer of
+ * ceil((edge_capacity + 3 (n_atoms + n_residues)) / 128) * 32 * hidden_nf floats, and dsb_dynamics_forward enqueues one
+ * more kernel per GCL sub-layer and per coordinate update (dsb_dynamics_last_launch_count counts them).  Status-flag
+ * semantics are unchanged.  Call it outside stream capture: a captured forward keeps the mode it was captured in. */
+int dsb_dynamics_set_deterministic(dsb_dynamics* dyn, int enable);
+
 /* ---- measurement hook (bench.py's live roofline).  When enabled, every non-captured forward brackets
  * its launches with CUDA events on the launch stream, grouped into 7 kernel classes:
  *   0 setup (plan, encoders+embedding, edge list)  1 node GEMMs  2 memsets  3 edge_gcl_kernel
