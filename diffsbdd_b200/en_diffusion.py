@@ -518,6 +518,22 @@ class EnVariationalDiffusion(nn.Module):
         st['sig'] = sig
         return g
 
+    def _graphed_joint_reverse_steps(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, first_s, n_steps, timesteps):
+        """Runs joint reverse steps s = first_s, first_s-1, ..., first_s-n_steps+1 by replaying one captured step (the
+        joint counterpart of ConditionalDDPM._graphed_reverse_steps)."""
+        dyn = self.dynamics
+        st = self._joint_engine(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, 1)
+        prev_defer, dyn.defer_status_check = dyn.defer_status_check, True
+        try:
+            g = self._joint_graph(st, 'reverse', z_lig, z_pocket, first_s)
+            st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
+            for _ in range(n_steps):
+                g.replay()
+        finally:
+            dyn.defer_status_check = prev_defer
+        dyn.check_status()
+        return st['zl'].clone(), st['zp'].clone()
+
     @follows_dynamics_determinism
     @torch.no_grad()
     def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu'):
@@ -532,21 +548,14 @@ class EnVariationalDiffusion(nn.Module):
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + z_pocket.size(), device=z_pocket.device)
         if self._joint_use_graph(z_lig.device):
-            dyn = self.dynamics
-            st = self._joint_engine(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, 1)
-            prev_defer, dyn.defer_status_check = dyn.defer_status_check, True
-            try:
-                g = self._joint_graph(st, 'reverse', z_lig, z_pocket, timesteps - 1)
-                st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(timesteps - 1)
-                for s in reversed(range(0, timesteps)):
-                    g.replay()
-                    if (s * return_frames) % timesteps == 0:
-                        idx = (s * return_frames) // timesteps
-                        out_lig[idx], out_pocket[idx] = self.unnormalize_z(st['zl'], st['zp'])
-            finally:
-                dyn.defer_status_check = prev_defer
-            dyn.check_status()
-            z_lig, z_pocket = st['zl'].clone(), st['zp'].clone()
+            stride = timesteps // return_frames       # frames are saved at s = idx * stride
+            s_hi = timesteps - 1
+            while s_hi >= 0:
+                s_lo = (s_hi // stride) * stride
+                z_lig, z_pocket = self._graphed_joint_reverse_steps(
+                    z_lig, z_pocket, lig_mask, pocket_mask, n_samples, s_hi, s_hi - s_lo + 1, timesteps)
+                out_lig[s_lo // stride], out_pocket[s_lo // stride] = self.unnormalize_z(z_lig, z_pocket)
+                s_hi = s_lo - 1
             self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         else:
             for s in reversed(range(0, timesteps)):

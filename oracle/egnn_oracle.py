@@ -161,13 +161,17 @@ def egnn_stack(sd, cfg, h, x, edges, update_coords_mask, batch_mask, edge_type_e
 
 def denoiser_forward(cfg, state_dict: Dict[str, torch.Tensor], xh_atoms, xh_residues, t,
                      mask_atoms, mask_residues, dtype=torch.float32,
-                     return_edges: bool = False, device='cpu'):
+                     return_edges: bool = False, device='cpu', edges=None):
     """``EGNNDynamics.forward`` (dynamics.py:87-167), eval mode, ``mode='egnn_dynamics'``.
 
     Returns ``(out_atoms [N_L,3+A], out_residues [N_P,3+R])`` on ``device`` (default CPU: the checker) in ``dtype``;
     raises ``ValueError('NaN detected in EGNN output')`` like dynamics.py:155-159.  ``device='cuda'`` runs the very same
     ATen op sequence on the GPU: that is bench.py's ``--impl reference-gpu`` arm ("the reference's own PyTorch graph on
-    the GPU", SURVEY.md §8(d)), never a checker and never the product path."""
+    the GPU", SURVEY.md §8(d)), never a checker and never the product path.
+
+    ``edges``: an int64 ``[2, E]`` edge list to evaluate on instead of ``build_edges`` (every edge must join two nodes of
+    one graph).  A float64 evaluation decides the cut-offs on float64 distances, which can differ from an fp32 decision
+    for pairs within a few ulp of a cut-off; passing the fp32 kernel's own edge list compares the two on the same graph."""
     if cfg.mode != 'egnn_dynamics':
         raise NotImplementedError('oracle covers mode=egnn_dynamics')
     sd = {k: v.detach().to(device, dtype) for k, v in state_dict.items()}
@@ -191,7 +195,10 @@ def denoiser_forward(cfg, state_dict: Dict[str, torch.Tensor], xh_atoms, xh_resi
             else:                                    # dynamics.py:110
                 h_time = t[mask]
             h = torch.cat([h, h_time], dim=1)
-        edges = build_edges(cfg, mask_atoms, mask_residues, x_lig, x_poc)
+        if edges is None:
+            edges = build_edges(cfg, mask_atoms, mask_residues, x_lig, x_poc)
+        else:
+            edges = edges.detach().to(device, torch.int64)
         assert torch.all(mask[edges[0]] == mask[edges[1]])       # dynamics.py:115
         emb = None
         if cfg.edge_embedding_dim:                                # dynamics.py:118-125
