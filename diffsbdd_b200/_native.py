@@ -18,8 +18,12 @@ EXPORTED_SYMBOLS = (
     'dsb_edge_capacity', 'dsb_dynamics_workspace_bytes', 'dsb_dynamics_forward', 'dsb_dynamics_edges',
     'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_deterministic', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
     'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_ddpm_noise',
-    'dsb_ddpm_vlb_terms', 'dsb_last_error', 'dsb_version',
+    'dsb_ddpm_vlb_terms', 'dsb_last_error', 'dsb_version', 'dsb_dynamics_set_stop_after', 'dsb_workspace_region',
 )
+
+# workspace regions of dsb_workspace_region (DSB_WS_* in include/diffsbdd_b200.h), in enum order
+WS_REGIONS = ('x_in', 'x_ping', 'x_pong', 'h', 'hT', 'agg', 'P', 'xagg', 'cent', 'deg', 'row_ptr', 'vrow_ptr', 'vmap',
+              'erow', 'ecol', 'ed0', 'part', 'lig_off', 'poc_off', 'gid', 'velmean')
 
 
 class DsbConfig(C.Structure):
@@ -106,8 +110,26 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dsb_ddpm_noise.restype = C.c_int
     lib.dsb_ddpm_vlb_terms.argtypes = [vp] * 16 + [i64, i64, i64, i32, i32, C.c_float, C.c_float, i32, vp, vp, vp]
     lib.dsb_ddpm_vlb_terms.restype = C.c_int
+    lib.dsb_dynamics_set_stop_after.argtypes = [vp, C.c_int]
+    lib.dsb_dynamics_set_stop_after.restype = C.c_int
+    lib.dsb_workspace_region.argtypes = [C.POINTER(DsbConfig), C.c_int, i64, i64, i64, i64, C.c_int, C.POINTER(i64),
+                                         C.POINTER(i64)]
+    lib.dsb_workspace_region.restype = C.c_int
     _LIB = lib
     return lib
+
+
+def workspace_regions(cfg: DsbConfig, deterministic: bool, n_atoms: int, n_residues: int, n_graphs: int,
+                      edge_capacity: int):
+    """{region name: (byte offset, bytes)} of the forward's workspace (dsb_workspace_region; test hook)."""
+    lib = load()
+    out = {}
+    off, nb = C.c_int64(), C.c_int64()
+    for i, name in enumerate(WS_REGIONS):
+        check(lib.dsb_workspace_region(C.byref(cfg), int(bool(deterministic)), n_atoms, n_residues, n_graphs,
+                                       edge_capacity, i, C.byref(off), C.byref(nb)))
+        out[name] = (off.value, nb.value)
+    return out
 
 
 def check(code: int) -> None:

@@ -307,34 +307,41 @@ static int pack_weights(dsb_dynamics* d, const float* const* params, const std::
 }
 
 // ---- workspace --------------------------------------------------------------------------------------------
-static Workspace carve(const dsb_config& c, int64_t NL, int64_t NP, int64_t B, int64_t Ecap, bool det, void* base) {
+// `regions` (optional, [DSB_WS_REGIONS][2]): receives (byte offset from base, bytes) of every region (dsb_workspace_region)
+static Workspace carve(const dsb_config& c, int64_t NL, int64_t NP, int64_t B, int64_t Ecap, bool det, void* base,
+                       int64_t (*regions)[2] = nullptr) {
   Workspace ws;
   const int64_t N = NL + NP;
   const int H = c.hidden_nf;
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~size_t(255); return base ? (char*)base + o : (char*)nullptr; };
-  ws.lig_off = (int32_t*)take(sizeof(int32_t) * (B + 2));
-  ws.poc_off = (int32_t*)take(sizeof(int32_t) * (B + 2));
-  ws.gid = (int32_t*)take(sizeof(int32_t) * (N + 1));
-  for (int i = 0; i < 3; ++i) ws.xbuf[i] = (float4*)take(sizeof(float4) * (N + 1));
-  ws.cent = (float4*)take(sizeof(float4) * (B + 1));
-  ws.xagg = (float4*)take(sizeof(float4) * (N + 1));
-  ws.velmean = (float4*)take(sizeof(float4) * (B + 1));
-  ws.h = (float*)take(sizeof(float) * (size_t)(N + 1) * H);
-  ws.hT = (float*)take(sizeof(float) * (size_t)(N + 257) * H);      // also the 3xFP16 operand image of h (whole 128-row tiles, one spare)
-  ws.agg = (float*)take(sizeof(float) * (size_t)(N + 1) * H);
-  ws.P = (float*)take(sizeof(float) * (size_t)(N + 1) * 6 * H);
-  ws.deg = (int32_t*)take(sizeof(int32_t) * (N + 1));
-  ws.row_ptr = (int32_t*)take(sizeof(int32_t) * (N + 2));
-  ws.vrow_ptr = (int32_t*)take(sizeof(int32_t) * (N + 2));
-  ws.vmap = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + (kRowChunk - 1) * N + 1));
-  ws.erow = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1));
-  ws.ecol = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1));
-  ws.ed0 = (float*)take(sizeof(float) * (size_t)(Ecap + 1));
+  auto take = [&](size_t bytes, int region) {
+    size_t o = off; off += (bytes + 255) & ~size_t(255);
+    if (regions) { regions[region][0] = (int64_t)o; regions[region][1] = (int64_t)bytes; }
+    return base ? (char*)base + o : (char*)nullptr;
+  };
+  ws.lig_off = (int32_t*)take(sizeof(int32_t) * (B + 2), DSB_WS_LIG_OFF);
+  ws.poc_off = (int32_t*)take(sizeof(int32_t) * (B + 2), DSB_WS_POC_OFF);
+  ws.gid = (int32_t*)take(sizeof(int32_t) * (N + 1), DSB_WS_GID);
+  for (int i = 0; i < 3; ++i) ws.xbuf[i] = (float4*)take(sizeof(float4) * (N + 1), DSB_WS_X_IN + i);
+  ws.cent = (float4*)take(sizeof(float4) * (B + 1), DSB_WS_CENT);
+  ws.xagg = (float4*)take(sizeof(float4) * (N + 1), DSB_WS_XAGG);
+  ws.velmean = (float4*)take(sizeof(float4) * (B + 1), DSB_WS_VELMEAN);
+  ws.h = (float*)take(sizeof(float) * (size_t)(N + 1) * H, DSB_WS_H);
+  ws.hT = (float*)take(sizeof(float) * (size_t)(N + 257) * H, DSB_WS_HT);      // also the 3xFP16 operand image of h (whole 128-row tiles, one spare)
+  ws.agg = (float*)take(sizeof(float) * (size_t)(N + 1) * H, DSB_WS_AGG);
+  ws.P = (float*)take(sizeof(float) * (size_t)(N + 1) * 6 * H, DSB_WS_P);
+  ws.deg = (int32_t*)take(sizeof(int32_t) * (N + 1), DSB_WS_DEG);
+  ws.row_ptr = (int32_t*)take(sizeof(int32_t) * (N + 2), DSB_WS_ROW_PTR);
+  ws.vrow_ptr = (int32_t*)take(sizeof(int32_t) * (N + 2), DSB_WS_VROW_PTR);
+  ws.vmap = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + (kRowChunk - 1) * N + 1), DSB_WS_VMAP);
+  ws.erow = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1), DSB_WS_EROW);
+  ws.ecol = (int32_t*)take(sizeof(int32_t) * (size_t)(Ecap + 1), DSB_WS_ECOL);
+  ws.ed0 = (float*)take(sizeof(float) * (size_t)(Ecap + 1), DSB_WS_ED0);
   // deterministic mode: one H-wide slot per 4-row chunk of the 128-row tiles that cover the virtual edge order (the
   // coordinate kernels use nm float4 per chunk, at most 8 floats <= H)
   const int64_t vtiles = (Ecap + (kRowChunk - 1) * N + 127) / 128;
-  ws.part = det ? (float*)take(sizeof(float) * (size_t)(vtiles * (128 / kRowChunk)) * H) : nullptr;
+  ws.part = det ? (float*)take(sizeof(float) * (size_t)(vtiles * (128 / kRowChunk)) * H, DSB_WS_PART) : nullptr;
+  if (!det && regions) { regions[DSB_WS_PART][0] = (int64_t)off; regions[DSB_WS_PART][1] = 0; }
   const int64_t vrows = Ecap + (kRowChunk - 1) * N;
   ws.vcap = (int32_t)(vrows < INT32_MAX ? vrows : INT32_MAX);
   ws.bytes = off;
@@ -826,7 +833,7 @@ static int setup(dsb_dynamics* dyn, int64_t n_atoms, int64_t n_residues, int64_t
   if (!dyn) { set_error("null handle"); return DSB_ERR_INVALID_ARGUMENT; }
   if (int e = check_sizes(n_atoms, n_residues, n_graphs, edge_capacity)) return e;
   if (!workspace) { set_error("null workspace"); return DSB_ERR_INVALID_ARGUMENT; }
-  char* base = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  char* base = (char*)(((uintptr_t)workspace + 255) & ~(uintptr_t)255);     // dsb_workspace_region assumes this alignment
   *ws = carve(dyn->cfg, n_atoms, n_residues, n_graphs, edge_capacity, dyn->deterministic != 0, base);
   if ((size_t)(base - (char*)workspace) + ws->bytes > workspace_bytes) {
     set_error("workspace too small: need %zu bytes, got %zu", ws->bytes + 256, workspace_bytes);
@@ -906,18 +913,29 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
     return ((mm & 1) && img.t_hi) ? launch_tc_node_gemm(dyn, ga, img, n_tile_off, f16, status, s) : launch_node_gemm(ga, s);
   };
 
+  // test hook (dsb_dynamics_set_stop_after): `ops` counts the operations enqueued so far; DSB_OP() before each one returns
+  // once the limit is reached.  `launches` keeps its own count (it is the reported launch count of a complete forward).
+  const int stop_at = dyn->stop_after;
+  int ops = 0;
+#define DSB_STOPPED() do { mark(-1); dyn->last_launches = ops - memsets; dyn->last_memsets = memsets; return 0; } while (0)
+#define DSB_OP() do { if (stop_at >= 0 && ops >= stop_at) DSB_STOPPED(); ++ops; } while (0)
+  auto budget = [&](int n) { return stop_at < 0 ? n : (stop_at - ops < n ? stop_at - ops : n); };
+
   mark(KC_SETUP);
-  DSB_TRY(launch_plan(dyn, dm, ws, mask_atoms, mask_residues, s)); launches += 1;
-  DSB_TRY(launch_prep(dyn, dm, ws, xh_atoms, xh_residues, t, t_numel, mask_atoms, mask_residues, false, s)); launches += 1;
-  DSB_TRY(launch_edges(dyn, dm, ws, status, s)); launches += 3;
+  DSB_OP(); DSB_TRY(launch_plan(dyn, dm, ws, mask_atoms, mask_residues, s)); launches += 1;
+  DSB_OP(); DSB_TRY(launch_prep(dyn, dm, ws, xh_atoms, xh_residues, t, t_numel, mask_atoms, mask_residues, false, s)); launches += 1;
+  {
+    const int n = budget(3);
+    DSB_TRY(launch_edges(dyn, dm, ws, status, s, n)); launches += 3; ops += n;
+    if (n < 3) DSB_STOPPED();
+  }
   const float4* xcur = ws.xbuf[0];
-  if (nm == 2) { mark(KC_COORD_FINISH); DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, nullptr, false, s)); launches += 1; }
+  if (nm == 2) { mark(KC_COORD_FINISH); DSB_OP(); DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, nullptr, false, s)); launches += 1; }
 
   // the aggregates are zeroed once here; afterwards each consumer re-arms them (node GEMM g3 zeroes agg, coord_finish zeroes xagg)
   mark(KC_MEMSET);
-  DSB_CUDA_OK(cudaMemsetAsync(ws.agg, 0, hbytes, s));
-  DSB_CUDA_OK(cudaMemsetAsync(ws.xagg, 0, sizeof(float4) * (size_t)dm.N, s));
-  memsets += 2;
+  DSB_OP(); DSB_CUDA_OK(cudaMemsetAsync(ws.agg, 0, hbytes, s)); memsets += 1;
+  DSB_OP(); DSB_CUDA_OK(cudaMemsetAsync(ws.xagg, 0, sizeof(float4) * (size_t)dm.N, s)); memsets += 1;
   // P buffer columns: [0, nq) = coordinate first layer of the current block (receiver block | sender block),
   // [nq, nq + 2H) = edge first layer (receiver | sender) of the GCL that runs next.
   const int nq = nm * 2 * H, ldP = nq + 2 * H, nrecv = nm * H;
@@ -929,22 +947,23 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
       if (!(sub == 0 && l > 0)) {      // otherwise produced by the previous block's merged GEMM
         mark(KC_NODE_GEMM);
         GemmArgs g1 = {ws.h, H, H, nullptr, 0, 0, 1.f, G.W1ab, 2 * H, G.b1ab, nullptr, 0, ws.P + nq, ldP, dm.N, 2 * H, 0, nullptr, 0, 0, 0};
-        DSB_TRY(gemm(g1, G.iW1ab));
+        DSB_OP(); DSB_TRY(gemm(g1, G.iW1ab));
         launches += 1;
       }
       mark(KC_EDGE_GCL);
+      DSB_OP();
       DSB_TRY((mm & 2) ? launch_tc_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, f16, status, s) : launch_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, s));
       if (det) {              // fixed-order receiver sums: agg = per-receiver sums of the chunk partials (one slot per chunk)
-        DSB_TRY(launch_segment_reduce(ws, dm.N, H / 4, 1, reinterpret_cast<float4*>(ws.agg), s));
+        DSB_OP(); DSB_TRY(launch_segment_reduce(ws, dm.N, H / 4, 1, reinterpret_cast<float4*>(ws.agg), s));
         launches += 1;
       }
       // node_model: h + W4 SiLU(W3 [h | agg/norm] + b3) + b4   (egnn_new.py:48-58)
       mark(KC_NODE_GEMM);
       GemmArgs g2 = {ws.h, H, H, ws.agg, H, H, c.normalization_factor, G.W3, H, G.b3, nullptr, 0, ws.hT, H, dm.N, H, 1, nullptr, 0, 0, 0,
                      c.aggregation_mean ? ws.deg : nullptr};
-      DSB_TRY(gemm(g2, G.iW3));
+      DSB_OP(); DSB_TRY(gemm(g2, G.iW3));
       GemmArgs g3 = {ws.hT, H, H, nullptr, 0, 0, 1.f, G.W4, H, G.b4, ws.h, H, ws.h, H, dm.N, H, 0, ws.agg, H, 0, 0};
-      DSB_TRY(gemm(g3, G.iW4));
+      DSB_OP(); DSB_TRY(gemm(g3, G.iW4));
       launches += 3;      // edge kernel, two node GEMMs
     }
     // one GEMM for everything that consumes the updated h: this block's coord/cross first layers and the next block's
@@ -953,22 +972,29 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
     mark(KC_NODE_GEMM);
     GemmArgs g4 = {ws.h, H, H, nullptr, 0, 0, 1.f, Q.W1, Q.nq + Q.np, Q.b1, nullptr, 0, ws.P, ldP, dm.N, Q.nq + Q.np, 0, nullptr, 0,
                    conditional ? dm.n_coord_rows : 0, conditional ? nrecv : 0};
-    DSB_TRY(gemm(g4, Q.iW1));
+    DSB_OP(); DSB_TRY(gemm(g4, Q.iW1));
     mark(KC_EDGE_COORD);
+    DSB_OP();
     DSB_TRY((mm & 4) ? launch_tc_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, f16, status, s) : launch_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, s));
     if (det && dm.n_coord_rows > 0) {   // xagg rows of the moving nodes; the tensor-core kernel keeps one slot per chunk and MLP
-      DSB_TRY(launch_segment_reduce(ws, dm.n_coord_rows, 1, (mm & 4) ? nm : 1, ws.xagg, s));
+      DSB_OP(); DSB_TRY(launch_segment_reduce(ws, dm.n_coord_rows, 1, (mm & 4) ? nm : 1, ws.xagg, s));
       launches += 1;
     }
     float4* xnext = ws.xbuf[1 + (l & 1)];
     mark(KC_COORD_FINISH);
-    DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, xnext, true, s));
+    DSB_OP(); DSB_TRY(launch_coord_finish(dyn, dm, ws, xcur, xnext, true, s));
     xcur = xnext;
     launches += 3;      // merged GEMM, coordinate edge kernel, finish
   }
   mark(KC_POST);
-  DSB_TRY(launch_post(dyn, dm, ws, xcur, out_atoms, out_residues, status, s));
+  {
+    const int np = c.update_pocket_coords ? 2 : 1, n = budget(np);
+    DSB_TRY(launch_post(dyn, dm, ws, xcur, out_atoms, out_residues, status, s, n)); ops += n;
+    if (n < np) DSB_STOPPED();
+  }
   mark(-1);
+#undef DSB_OP
+#undef DSB_STOPPED
 #undef DSB_TRY
   launches += 1 + (c.update_pocket_coords ? 1 : 0);
   dyn->last_launches = launches;
@@ -1025,6 +1051,25 @@ int dsb_dynamics_collect_profile(dsb_dynamics* dyn, double* ms_by_class, int64_t
 }
 
 int dsb_dynamics_last_launch_count(const dsb_dynamics* dyn) { return dyn ? dyn->last_launches : 0; }
+
+int dsb_dynamics_set_stop_after(dsb_dynamics* dyn, int n_ops) {
+  if (!dyn) { set_error("null handle"); return DSB_ERR_INVALID_ARGUMENT; }
+  const int old = dyn->stop_after;
+  dyn->stop_after = n_ops < 0 ? -1 : n_ops;
+  return old;
+}
+
+int dsb_workspace_region(const dsb_config* cfg, int deterministic, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                         int64_t edge_capacity, int region, int64_t* offset, int64_t* bytes) {
+  if (int e = validate(cfg)) return e;
+  if (int e = check_sizes(n_atoms, n_residues, n_graphs, edge_capacity)) return e;
+  if (region < 0 || region >= DSB_WS_REGIONS || !offset || !bytes) { set_error("bad workspace region %d", region); return DSB_ERR_INVALID_ARGUMENT; }
+  int64_t reg[DSB_WS_REGIONS][2] = {};
+  carve(*cfg, n_atoms, n_residues, n_graphs, edge_capacity, deterministic != 0, nullptr, reg);
+  *offset = reg[region][0];
+  *bytes = reg[region][1];
+  return 0;
+}
 
 int dsb_ddpm_ligand_update(const float* z_lig, const float* eps_hat, const float* noise, const float* coef,
                            const int64_t* mask_atoms, const int64_t* mask_residues, const float* xh_pocket,

@@ -121,6 +121,7 @@ struct dsb_dynamics {
   int deterministic = 0;     // 1: fixed-order receiver sums (chunk partials + segment reduce) instead of atomics
   int last_launches = 0;     // kernels only
   int last_memsets = 0;
+  int stop_after = -1;       // test hook (dsb_dynamics_set_stop_after): forward enqueues only its first stop_after operations
   // profiling
   int prof_enabled = 0;
   cudaEvent_t* prof_ev = nullptr;      // [2 * kMaxProfEvents]
@@ -188,11 +189,14 @@ int launch_plan(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, cons
 int launch_prep(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const float* xh_atoms,
                 const float* xh_residues, const float* t, int64_t t_numel, const int64_t* mask_atoms,
                 const int64_t* mask_residues, bool coords_only, cudaStream_t s);
-int launch_edges(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, int32_t* status, cudaStream_t s);
+// launch_edges enqueues 3 kernels (count, scan, fill) and launch_post 2 in joint mode (velocity mean, decoders), else 1;
+// max_launches < that stops after the first max_launches of them (dsb_dynamics_set_stop_after)
+int launch_edges(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, int32_t* status, cudaStream_t s,
+                 int max_launches = 3);
 int launch_coord_finish(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const float4* x_old,
                         float4* x_new, bool apply_update, cudaStream_t s);
 int launch_post(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const float4* x_final,
-                float* out_atoms, float* out_residues, int32_t* status, cudaStream_t s);
+                float* out_atoms, float* out_residues, int32_t* status, cudaStream_t s, int max_launches = 2);
 
 // ---- launchers implemented in dsb_edge.cu ----------------------------------------------------------
 struct PView { const float* P; int ldp; };           // where an edge kernel finds its factorised first-layer outputs

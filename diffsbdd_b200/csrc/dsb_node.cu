@@ -261,7 +261,8 @@ __global__ void __launch_bounds__(1024) scan_kernel(const int32_t* __restrict__ 
   }
 }
 
-int launch_edges(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, int32_t* status, cudaStream_t s) {
+int launch_edges(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, int32_t* status, cudaStream_t s,
+                 int max_launches) {
   const dsb_config& c = d->cfg;
   EdgeBuildArgs a;
   a.x = ws.xbuf[0]; a.gid = ws.gid; a.lig_off = ws.lig_off; a.poc_off = ws.poc_off;
@@ -271,9 +272,9 @@ int launch_edges(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, int
   a.vrow_ptr = ws.vrow_ptr; a.vmap = ws.vmap;
   const int blocks = (dm.N * 32 + 255) / 256;
   if (dm.N == 0) return 0;
-  DSB_CUDA_OK(launch_k(edge_rows_kernel<false>, blocks, 256, 0, s, a));
-  DSB_CUDA_OK(launch_k(scan_kernel, 1, 1024, 0, s, ws.deg, ws.row_ptr, ws.vrow_ptr, dm.N, dm.Ecap, status));
-  DSB_CUDA_OK(launch_k(edge_rows_kernel<true>, blocks, 256, 0, s, a));
+  if (max_launches > 0) DSB_CUDA_OK(launch_k(edge_rows_kernel<false>, blocks, 256, 0, s, a));
+  if (max_launches > 1) DSB_CUDA_OK(launch_k(scan_kernel, 1, 1024, 0, s, ws.deg, ws.row_ptr, ws.vrow_ptr, dm.N, dm.Ecap, status));
+  if (max_launches > 2) DSB_CUDA_OK(launch_k(edge_rows_kernel<true>, blocks, 256, 0, s, a));
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -466,13 +467,16 @@ __global__ void __launch_bounds__(PREP_THREADS) post_kernel(PostArgs p) {
 }
 
 int launch_post(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const float4* x_final,
-                float* out_atoms, float* out_residues, int32_t* status, cudaStream_t s) {
+                float* out_atoms, float* out_residues, int32_t* status, cudaStream_t s, int max_launches) {
   const dsb_config& c = d->cfg;
   const PackedWeights& w = d->w;
   static_assert(POST_NPW == 4, "lane select below assumes 4 nodes per warp");
   if (c.update_pocket_coords && dm.B > 0) {
+    if (max_launches < 1) return 0;
     DSB_CUDA_OK(launch_k(velmean_kernel, dm.B, 128, 0, s, x_final, ws.xbuf[0], ws.lig_off, ws.poc_off, dm.NL, ws.velmean));
+    --max_launches;
   }
+  if (max_launches < 1) return 0;
   PostArgs p;
   p.h = ws.h; p.x_fin = x_final; p.x_in = ws.xbuf[0]; p.gid = ws.gid; p.velmean = ws.velmean;
   p.NL = dm.NL; p.NP = dm.NP; p.A = c.atom_nf; p.R = c.residue_nf; p.H = c.hidden_nf; p.joint = c.update_pocket_coords;

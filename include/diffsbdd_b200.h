@@ -125,6 +125,38 @@ int dsb_dynamics_edges(dsb_dynamics* dyn,
 /* Number of kernel launches (memsets excluded) the last dsb_dynamics_forward on this module enqueued. */
 int dsb_dynamics_last_launch_count(const dsb_dynamics* dyn);
 
+/* ---- test hooks (host only; they change no kernel).  They let a test stop the forward after any operation and read its
+ * workspace, so that every launch can be checked on its own against a float64 restatement of what it computes.
+ *
+ * dsb_dynamics_set_stop_after: afterwards dsb_dynamics_forward enqueues only its first n_ops operations (kernel launches
+ * and memsets, counted in the fixed order the forward enqueues them) and returns 0.  A negative n_ops means no limit (the
+ * default).  Returns the previous setting.  When the forward stops early, out_atoms / out_residues and status are not
+ * written (except status[1] and [2] by the edge-list scan if it ran), and dsb_dynamics_last_launch_count counts the
+ * launches that were enqueued.  Not for production use: a stopped forward computes nothing a caller can use. */
+int dsb_dynamics_set_stop_after(dsb_dynamics* dyn, int n_ops);
+
+/* dsb_workspace_region: byte offset and size of one region of the forward's workspace for the given config, mode
+ * (deterministic 0/1) and sizes, as dsb_dynamics_forward lays it out.  The offset is from a workspace pointer aligned to
+ * 256 bytes (the forward rounds the pointer it is given up to that alignment; caching allocators return such pointers).
+ * N = n_atoms + n_residues, B = n_graphs, H = hidden_nf, nm = 2 without reflection equivariance, else 1:
+ *   X_IN, X_PING, X_PONG  float4 [N + 1]  (x, y, z, 0) per node: input coordinates, then the blocks' outputs alternating
+ *   H, HT, AGG            float [N + 1][H] (HT: N + 257 rows): node features, node-MLP hidden layer, raw receiver sums
+ *   P                     float [N + 1][6 H]; the forward uses leading dimension (2 nm + 2) H: [coord/cross receiver |
+ *                         coord/cross sender | next edge MLP receiver | sender] first-layer outputs
+ *   XAGG, CENT, VELMEAN   float4 [N + 1], [B + 1], [B + 1]: raw coordinate sums, per-graph centroids, velocity means
+ *   DEG, ROW_PTR, VROW_PTR int32 [N + 1], [N + 2], [N + 2];  VMAP int32 [edge_capacity + 3 N + 1]
+ *   EROW, ECOL, ED0       int32 / int32 / float [edge_capacity + 1]: CSR edges and their input-geometry d^2
+ *   PART                  deterministic mode only (0 bytes otherwise): per-chunk partial sums
+ *   LIG_OFF, POC_OFF, GID int32 [B + 2], [B + 2], [N + 1]
+ * Returns 0, or a negative dsb_status for a bad config, size or region. */
+enum {
+  DSB_WS_X_IN = 0, DSB_WS_X_PING, DSB_WS_X_PONG, DSB_WS_H, DSB_WS_HT, DSB_WS_AGG, DSB_WS_P, DSB_WS_XAGG, DSB_WS_CENT,
+  DSB_WS_DEG, DSB_WS_ROW_PTR, DSB_WS_VROW_PTR, DSB_WS_VMAP, DSB_WS_EROW, DSB_WS_ECOL, DSB_WS_ED0, DSB_WS_PART,
+  DSB_WS_LIG_OFF, DSB_WS_POC_OFF, DSB_WS_GID, DSB_WS_VELMEAN, DSB_WS_REGIONS
+};
+int dsb_workspace_region(const dsb_config* cfg, int deterministic, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                         int64_t edge_capacity, int region, int64_t* offset, int64_t* bytes);
+
 /* Process-wide switch for programmatic dependent launch of the forward's kernels (each kernel's launch and prologue
  * overlap its predecessor's tail; every kernel executes griddepcontrol.wait before touching data a predecessor may
  * have written).  enable: 1 on, 0 off, negative = query only.  Returns the previous setting.  Initial value: the
@@ -153,7 +185,8 @@ int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode);
  * programmatic dependent launch, workspace / output addresses and the persistent grid size.  A graph's outputs do not
  * depend bitwise on the other graphs of the batch only in math mode 0 (fp32 FFMA kernels); with any tensor-core kernel
  * (math mode != 0) the same graph denoised alone and inside another batch can differ in the last bits (measured up to
- * ~2e-6), so regenerating one graph bit for bit needs the same batch layout as well.  Results are not bit-identical
+ * ~2e-6: the tensor-core edge kernels' SiLU shares one reciprocal between tile rows r and r + 8, so an edge's rounding
+ * depends on the edge 8 rows away), so regenerating one graph bit for bit needs the same batch layout as well.  Results are not bit-identical
  * across math modes, nor with the default mode.  If the edges of a call exceed edge_capacity (status[2]) the outputs are
  * invalid as in the default mode; the deterministic kernels then stop at the end of the partial buffer.  Cost: dsb_dynamics_workspace_bytes grows by a partial buffer of
  * ceil((edge_capacity + 3 (n_atoms + n_residues)) / 128) * 32 * hidden_nf floats, and dsb_dynamics_forward enqueues one
