@@ -189,8 +189,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
       wgmma_fence();
       mma_chunk<F16, H>(acc, st, wg, kc == 0);
       wgmma_commit();
-      trk.after_commit<H>(ctl, acc, (int)q, kc == chunks - 1, lane == 0);
+      trk.release_prev(ctl, (int)q, lane == 0);
     }
+    trk.drain<H>(ctl, acc, lane == 0);
     // epilogue from registers: rows re, re + 8; columns 8j + 2 (lane % 4) + {0, 1}
     const f32x2 ip = pk2(g.inv_scale, g.inv_scale);
 #pragma unroll
@@ -226,13 +227,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
 // =====================================================================================================
 // edge kernels
 // =====================================================================================================
+struct EdgeScalars {          // per-edge scalars of one unit (virtual row order)
+  float d2[TM], d0[TM];
+  int row[TM], col[TM], type[TM];
+  float dir[3][TM];           // coord: direction of this MLP's term
+};
+
 template <int H>
 struct EdgeExtra {            // shared memory after Control
   float vec[2][3 * H];        // per MLP: wr, wr0, b2   (the edge-type table tb stays in global/L1)
   float wa[H];                // attention weight (GCL) or w3 (coord)
-  float d2[TM], d0[TM];       // per-edge scalars of the current tile
-  int row[TM], col[TM], type[TM];
-  float dir[3][TM];           // coord: direction of this MLP's term
+  EdgeScalars sc[2];          // unit j uses sc[j & 1]; unit j + 1's are written while unit j is on the tensor pipe
 };
 
 struct TcEdgeArgs {
@@ -252,39 +257,54 @@ struct TcEdgeArgs {
   int vcap;                                  // deterministic variant: virtual rows covered by vmap / part (Workspace::vcap)
 };
 
-// per-edge scalars of edge tile v0/TM for MLP m (thread pr handles virtual row v0 + pr)
-template <bool COORD, int H>
-__device__ __forceinline__ void edge_scalars(const TcEdgeArgs& a, EdgeExtra<H>* ex, int pr, int v0, int V, int m) {
-  const int vr = v0 + pr;
-  const int e = vr < V ? a.vmap[vr] : -1;
-  int r = -1, c = 0, ty = 0; float d2 = 0.f, d0 = 0.f;
-  float dir[3] = {0.f, 0.f, 0.f};
-  if (e >= 0) {
-    r = a.erow[e]; c = a.ecol[e]; d0 = a.ed0[e];
-    const float4 xi = a.x[r], xj = a.x[c];
-    const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
-    d2 = dx * dx + dy * dy + dz * dz;
-    ty = (r < a.NL) == (c < a.NL) ? (r < a.NL ? 1 : 2) : 0;
-    if (COORD) {
-      if (m == 0) {                                                     // egnn_new.py:300-301 (coord2diff)
-        const float den = sqrtf(d2 + 1e-8f) + a.norm_constant;
-        dir[0] = dx / den; dir[1] = dy / den; dir[2] = dz / den;
-      } else {                                                          // egnn_new.py:312-315 (coord2cross)
-        const float4 mu = a.cent[a.gid[r]];
-        const float ax = xi.x - mu.x, ay = xi.y - mu.y, az = xi.z - mu.z;
-        const float bx = xj.x - mu.x, by = xj.y - mu.y, bz = xj.z - mu.z;
-        const float cx = ay * bz - az * by, cy = az * bx - ax * bz, cz = ax * by - ay * bx;
-        const float cn = sqrtf(cx * cx + cy * cy + cz * cz) + a.norm_constant;
-        dir[0] = cx / cn; dir[1] = cy / cn; dir[2] = cz / cn;
+// Per-edge scalars of the unit at virtual row v0 for MLP m (thread pr handles virtual row v0 + pr), produced in four steps
+// that each wait for the loads of the one before: 0 vmap, 1 edge ids and d0, 2 coordinates (and graph id), 3 centroid,
+// finish and store.  The edge kernel runs the steps of the next unit between the chunks of the current one, so each load's
+// latency hides under a chunk of wgmmas.  Branch-free (clamped indices, selects): it runs inside the wgmma window.
+// Rows past V and pad rows (vmap -1) get row -1 and zero scalars.
+template <bool COORD>
+struct ScalarSteps {
+  int e, r, c, gi;
+  float d0;
+  float4 xi, xj;
+  __device__ __forceinline__ void step(int k, const TcEdgeArgs& a, EdgeScalars* sc, int pr, int v0, int V, int m) {
+    if (k == 0) {
+      const int vr = v0 + pr;
+      e = a.vmap[min(vr, V - 1)];
+      e = vr < V ? e : -1;
+    } else if (k == 1) {
+      const int ec = max(e, 0);
+      r = a.erow[ec]; c = a.ecol[ec]; d0 = a.ed0[ec];
+      r = e >= 0 ? r : 0; c = e >= 0 ? c : 0;
+    } else if (k == 2) {
+      xi = a.x[r]; xj = a.x[c];
+      if (COORD) gi = a.gid[r];
+    } else {
+      const bool live = e >= 0;
+      const float dx = xi.x - xj.x, dy = xi.y - xj.y, dz = xi.z - xj.z;
+      const float d2 = dx * dx + dy * dy + dz * dz;
+      const int ty = (r < a.NL) == (c < a.NL) ? (r < a.NL ? 1 : 2) : 0;
+      sc->row[pr] = live ? r : -1; sc->col[pr] = c; sc->d2[pr] = live ? d2 : 0.f; sc->d0[pr] = live ? d0 : 0.f;
+      sc->type[pr] = live ? ty : 0;
+      if (COORD) {
+        float dir[3];
+        if (m == 0) {                                                   // egnn_new.py:300-301 (coord2diff)
+          const float den = sqrtf(d2 + 1e-8f) + a.norm_constant;
+          dir[0] = dx / den; dir[1] = dy / den; dir[2] = dz / den;
+        } else {                                                        // egnn_new.py:312-315 (coord2cross)
+          const float4 mu = a.cent[gi];
+          const float ax = xi.x - mu.x, ay = xi.y - mu.y, az = xi.z - mu.z;
+          const float bx = xj.x - mu.x, by = xj.y - mu.y, bz = xj.z - mu.z;
+          const float cx = ay * bz - az * by, cy = az * bx - ax * bz, cz = ax * by - ay * bx;
+          const float cn = sqrtf(cx * cx + cy * cy + cz * cz) + a.norm_constant;
+          dir[0] = cx / cn; dir[1] = cy / cn; dir[2] = cz / cn;
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) sc->dir[k][pr] = live ? dir[k] : 0.f;
       }
     }
   }
-  ex->row[pr] = r; ex->col[pr] = c; ex->d2[pr] = d2; ex->d0[pr] = d0; ex->type[pr] = ty;
-  if (COORD) {
-#pragma unroll
-    for (int k = 0; k < 3; ++k) ex->dir[k][pr] = dir[k];
-  }
-}
+};
 
 // Work unit = virtual tile v = edge_tile * nm + m (the m-th MLP over 128 virtual edge rows).  The coordinate update is a sum
 // of independent terms per MLP (egnn_new.py:100-109: trans = diff * f(phi) + cross * f(phi_x)), so the two MLPs of an edge tile
@@ -354,64 +374,87 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
   const int re = wg * WG_ROWS + 16 * warp + (lane >> 2);   // accumulator rows re, re + 8
   const float* const Pt = a.P + 4 * pc;
   const int soff = nm * H;                   // sender block follows the nm receiver blocks
-  float acc[G::ACC];
-  MmaTracker trk;
-  uint32_t q = 0;
-  for (int j = 0; j < n_my; ++j) {
-    int m;
-    const int e0 = unit_tile(j, m) * TM;
-    wg_sync(wg);                               // the previous unit's epilogue is done with this warpgroup's scalars
-    if (wt < WG_ROWS) edge_scalars<COORD, H>(a, ex, wg * WG_ROWS + wt, e0, E, m);
-    wg_sync(wg);
+  // A operand of K-chunk kc of the unit with scalars sc and MLP m into stage s
+  auto build = [&](const EdgeScalars* sc, int m, int kc, int s) {
+    char* st = stages + (size_t)s * G::STAGE_BYTES;
     const int moff = m * H;
-    const float* pr = Pt + (size_t)max(ex->row[r0], 0) * a.ldp + moff;
-    const float* ps[4];
-    float pd2[4], pd0[4];
-    int pty[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      ps[i] = Pt + (size_t)ex->col[r0 + i] * a.ldp + (soff + moff);
-      pd2[i] = ex->d2[r0 + i]; pd0[i] = ex->d0[r0 + i];
-      pty[i] = TB ? ex->type[r0 + i] * H : 0;
-    }
+    const float* pr = Pt + (size_t)max(sc->row[r0], 0) * a.ldp + moff;
+    const int4 cl = *reinterpret_cast<const int4*>(sc->col + r0);
+    const float4 d2v = *reinterpret_cast<const float4*>(sc->d2 + r0), d0v = *reinterpret_cast<const float4*>(sc->d0 + r0);
+    const int4 tyv = *reinterpret_cast<const int4*>(sc->type + r0);
+    const float* const ps[4] = {Pt + (size_t)cl.x * a.ldp + (soff + moff), Pt + (size_t)cl.y * a.ldp + (soff + moff),
+                                Pt + (size_t)cl.z * a.ldp + (soff + moff), Pt + (size_t)cl.w * a.ldp + (soff + moff)};
+    const float pd2[4] = {d2v.x, d2v.y, d2v.z, d2v.w}, pd0[4] = {d0v.x, d0v.y, d0v.z, d0v.w};
+    const int pty[4] = {TB ? tyv.x * H : 0, TB ? tyv.y * H : 0, TB ? tyv.z * H : 0, TB ? tyv.w * H : 0};
     const float* wr = ex->vec[m] + 4 * pc;
     const float* wr0 = wr + H;
     const float* tbm = TB ? a.tb[m] + 4 * pc : nullptr;
-#pragma unroll 1
-    for (int kc = 0; kc < chunks; ++kc, ++q) {
-      const int s = q & 1;
-      char* st = stages + (size_t)s * G::STAGE_BYTES;
 #pragma unroll
-      for (int h = 0; h < HPC; ++h) {
-        const int hf = kc * HPC + h;
-        const float4 ga = *reinterpret_cast<const float4*>(pr + hf * TKC);
-        float4 gb[4];
+    for (int h = 0; h < HPC; ++h) {
+      const int hf = kc * HPC + h;
+      const float4 ga = *reinterpret_cast<const float4*>(pr + hf * TKC);
+      float4 gb[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) gb[i] = *reinterpret_cast<const float4*>(ps[i] + hf * TKC);
-        const float4 r4 = *reinterpret_cast<const float4*>(wr + hf * TKC);
-        const float4 r04 = *reinterpret_cast<const float4*>(wr0 + hf * TKC);
-        const f32x2 a01 = pk2(ga.x, ga.y), a23 = pk2(ga.z, ga.w);
+      for (int i = 0; i < 4; ++i) gb[i] = *reinterpret_cast<const float4*>(ps[i] + hf * TKC);
+      const float4 r4 = *reinterpret_cast<const float4*>(wr + hf * TKC);
+      const float4 r04 = *reinterpret_cast<const float4*>(wr0 + hf * TKC);
+      const f32x2 a01 = pk2(ga.x, ga.y), a23 = pk2(ga.z, ga.w);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const f32x2 d2p = pk2(pd2[i], pd2[i]), d0p = pk2(pd0[i], pd0[i]);
-          f32x2 u01 = fma2(d0p, pk2(r04.x, r04.y), fma2(d2p, pk2(r4.x, r4.y), add2(a01, pk2(gb[i].x, gb[i].y))));
-          f32x2 u23 = fma2(d0p, pk2(r04.z, r04.w), fma2(d2p, pk2(r4.z, r4.w), add2(a23, pk2(gb[i].z, gb[i].w))));
-          if (TB) {
-            const float4 t4 = *reinterpret_cast<const float4*>(tbm + pty[i] + hf * TKC);
-            u01 = add2(u01, pk2(t4.x, t4.y)); u23 = add2(u23, pk2(t4.z, t4.w));
-          }
-          silu_pair<(DSB_SILU_PAIR & 1) != 0, (DSB_SILU_QUAD & 1) != 0>(u01, u23);
-          store_pair<F16>(st + piece_offset<F16>(r0 + i, hf, pc), u01, u23);
+      for (int i = 0; i < 4; ++i) {
+        const f32x2 d2p = pk2(pd2[i], pd2[i]), d0p = pk2(pd0[i], pd0[i]);
+        f32x2 u01 = fma2(d0p, pk2(r04.x, r04.y), fma2(d2p, pk2(r4.x, r4.y), add2(a01, pk2(gb[i].x, gb[i].y))));
+        f32x2 u23 = fma2(d0p, pk2(r04.z, r04.w), fma2(d2p, pk2(r4.z, r4.w), add2(a23, pk2(gb[i].z, gb[i].w))));
+        if (TB) {
+          const float4 t4 = *reinterpret_cast<const float4*>(tbm + pty[i] + hf * TKC);
+          u01 = add2(u01, pk2(t4.x, t4.y)); u23 = add2(u23, pk2(t4.z, t4.w));
         }
+        silu_pair<(DSB_SILU_PAIR & 1) != 0, (DSB_SILU_QUAD & 1) != 0>(u01, u23);
+        store_pair<F16>(st + piece_offset<F16>(r0 + i, hf, pc), u01, u23);
       }
-      fence_proxy_async();
-      wg_sync(wg);
-      mbar_wait(&ctl->full_w[s], (q >> 1) & 1);
-      wgmma_fence();
-      mma_chunk<F16, H>(acc, st, wg, kc == 0);
-      wgmma_commit();
-      trk.after_commit<H>(ctl, acc, (int)q, kc == chunks - 1, lane == 0);
     }
+  };
+  float acc[G::ACC];
+  MmaTracker trk;
+  uint32_t q = 0;
+  // issue the wgmmas of chunk kc (global chunk q, built into stage q & 1)
+  auto issue = [&](int kc) {
+    const int s = q & 1;
+    fence_proxy_async();
+    wg_sync(wg);
+    mbar_wait(&ctl->full_w[s], (q >> 1) & 1);
+    wgmma_fence();
+    mma_chunk<F16, H>(acc, stages + (size_t)s * G::STAGE_BYTES, wg, kc == 0);
+    wgmma_commit();
+    trk.release_prev(ctl, (int)q, lane == 0);
+    ++q;
+  };
+  // Unit pipeline: unit j + 1's scalars are produced into sc[(j + 1) & 1] step by step after chunks 0 .. chunks - 2 of unit
+  // j have been issued, and its chunk 0 is built under unit j's last chunk; only the epilogue runs with no wgmma in flight.
+  // Both threads of a row pair (wt, wt + 64) produce the row's scalars (same values): no thread-dependent branch.
+  static_assert(chunks >= 2, "the scalar steps of the next unit need at least one chunk before the last");
+  constexpr int kSteps = 4;
+  const int psc = wg * WG_ROWS + (wt & (WG_ROWS - 1));
+  ScalarSteps<COORD> stp;
+  int m;
+  int e0 = unit_tile(0, m) * TM;
+  for (int k = 0; k < kSteps; ++k) stp.step(k, a, &ex->sc[0], psc, e0, E, m);
+  wg_sync(wg);
+  build(&ex->sc[0], m, 0, 0);
+  for (int j = 0; j < n_my; ++j) {
+    const EdgeScalars* sc = &ex->sc[j & 1];
+    EdgeScalars* sc_next = &ex->sc[(j + 1) & 1];
+    int m_next;
+    const int e0_next = unit_tile(j + 1, m_next) * TM;      // past the last unit: rows >= E, all padding
+#pragma unroll (F16 ? chunks : 1)
+    for (int kc = 0; kc < chunks - 1; ++kc) {
+      issue(kc);
+      for (int k = kc * kSteps / (chunks - 1); k < (kc + 1) * kSteps / (chunks - 1); ++k)
+        stp.step(k, a, sc_next, psc, e0_next, E, m_next);
+      build(sc, m, kc + 1, q & 1);
+    }
+    issue(chunks - 1);
+    build(sc_next, m_next, 0, q & 1);
+    trk.drain<H>(ctl, acc, lane == 0);
 
     // ---- epilogue, pass 1: m = SiLU(acc * inv + b2) in place; s = wa . m per row
     const float* b2 = ex->vec[m] + 2 * H;
@@ -432,39 +475,42 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
     }
     s_lo += __shfl_xor_sync(0xffffffffu, s_lo, 1); s_lo += __shfl_xor_sync(0xffffffffu, s_lo, 2);
     s_hi += __shfl_xor_sync(0xffffffffu, s_hi, 1); s_hi += __shfl_xor_sync(0xffffffffu, s_hi, 2);
-    const int row_lo = ex->row[re], row_hi = ex->row[re + 8];
-    const int crow_lo = ex->row[re & ~3], crow_hi = ex->row[(re + 8) & ~3];     // receiver of the row's 4-row chunk
+    const int row_lo = sc->row[re], row_hi = sc->row[re + 8];
+    const int crow_lo = sc->row[re & ~3], crow_hi = sc->row[(re + 8) & ~3];     // receiver of the row's 4-row chunk
     const bool chunk_lane = (lane & 12) == 0;                                   // first row of its chunk
     if constexpr (!COORD) {
-      // ---- pass 2: gate-weighted messages, 4-row chunk sums, one vector RED per chunk and column pair
+      // ---- pass 2: gate-weighted messages, 4-row chunk sums (reduce-scatter), one vector RED per lane and column-group pair
       // pad rows share a chunk with real rows: weight 0 (selects, not branches: a divergent path next to the accumulator
       // registers makes the compiler serialise the wgmmas)
       float g_lo = has_att ? sigmoid_f(s_lo + ba) : 1.0f, g_hi = has_att ? sigmoid_f(s_hi + ba) : 1.0f;
       g_lo = row_lo >= 0 ? g_lo : 0.f;
       g_hi = row_hi >= 0 ? g_hi : 0.f;
-      float* const dst_lo = DET ? a.part + (size_t)((e0 + (re & ~3)) / kRowChunk) * H + 2 * (lane & 3)
-                                : a.agg + (size_t)max(crow_lo, 0) * H + 2 * (lane & 3);
-      float* const dst_hi = DET ? a.part + (size_t)((e0 + ((re + 8) & ~3)) / kRowChunk) * H + 2 * (lane & 3)
-                                : a.agg + (size_t)max(crow_hi, 0) * H + 2 * (lane & 3);
+      // The four lanes of a chunk (lanes 4 and 8 apart) hold rows re (chunk lo) and re + 8 (chunk hi) of two column groups
+      // jj, jj + 1: 8 values each.  Lanes 4 apart (rows 0|1, 2|3 of the chunks) swap halves and add: the lane with
+      // (lane & 4) == 0 keeps chunk lo, its partner chunk hi.  Lanes 8 apart (row pairs {0,1}|{2,3}) swap again: the lane
+      // with (lane & 8) == 0 keeps group jj, its partner group jj + 1.  Every lane ends with one finished column pair, summed
+      // (x0 + x1) + (x2 + x3) over the chunk's rows as by the all-reduce this replaces.
+      const bool hi_half = (lane & 4) != 0, odd_group = (lane & 8) != 0;
+      const int crow = hi_half ? crow_hi : crow_lo;
+      const int chunk_row = hi_half ? (re + 8) & ~3 : re & ~3;
+      float* const dst = (DET ? a.part + (size_t)((e0 + chunk_row) / kRowChunk) * H : a.agg + (size_t)max(crow, 0) * H)
+                         + 2 * (lane & 3) + (odd_group ? 8 : 0);
 #pragma unroll
-      for (int jj = 0; jj < H / 8; ++jj) {
-        float v0 = g_lo * acc[4 * jj], v1 = g_lo * acc[4 * jj + 1], v2 = g_hi * acc[4 * jj + 2], v3 = g_hi * acc[4 * jj + 3];
-        v0 += __shfl_xor_sync(0xffffffffu, v0, 4); v1 += __shfl_xor_sync(0xffffffffu, v1, 4);
-        v2 += __shfl_xor_sync(0xffffffffu, v2, 4); v3 += __shfl_xor_sync(0xffffffffu, v3, 4);
-        v0 += __shfl_xor_sync(0xffffffffu, v0, 8); v1 += __shfl_xor_sync(0xffffffffu, v1, 8);
-        v2 += __shfl_xor_sync(0xffffffffu, v2, 8); v3 += __shfl_xor_sync(0xffffffffu, v3, 8);
-        // one lane per chunk (predicated, not a branch); a chunk of padding only has gate 0 on all rows: its sums are exactly
-        // 0 and go to row 0 (DET: to the pad chunk's own slot, which no receiver reads)
+      for (int jj = 0; jj < H / 8; jj += 2) {
+        const float lo[4] = {g_lo * acc[4 * jj], g_lo * acc[4 * jj + 1], g_lo * acc[4 * jj + 4], g_lo * acc[4 * jj + 5]};
+        const float hi[4] = {g_hi * acc[4 * jj + 2], g_hi * acc[4 * jj + 3], g_hi * acc[4 * jj + 6], g_hi * acc[4 * jj + 7]};
+        float t[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) t[k] = (hi_half ? hi[k] : lo[k]) + __shfl_xor_sync(0xffffffffu, hi_half ? lo[k] : hi[k], 4);
+        float u[2];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) u[k] = (odd_group ? t[2 + k] : t[k]) + __shfl_xor_sync(0xffffffffu, odd_group ? t[k] : t[2 + k], 8);
+        // a chunk of padding only has gate 0 on all rows: its sums are exactly 0 and go to row 0 (DET: to the pad chunk's
+        // own slot, which no receiver reads)
         if constexpr (DET)
-          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
-                       "@p st.global.v2.f32 [%0], {%1, %2};\n\t"
-                       "@p st.global.v2.f32 [%3], {%4, %6};\n\t}"
-                       ::"l"(dst_lo + 8 * jj), "f"(v0), "f"(v1), "l"(dst_hi + 8 * jj), "f"(v2), "r"((int)chunk_lane), "f"(v3) : "memory");
+          asm volatile("st.global.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj), "f"(u[0]), "f"(u[1]) : "memory");
         else
-          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
-                       "@p red.global.add.v2.f32 [%0], {%1, %2};\n\t"
-                       "@p red.global.add.v2.f32 [%3], {%4, %6};\n\t}"
-                       ::"l"(dst_lo + 8 * jj), "f"(v0), "f"(v1), "l"(dst_hi + 8 * jj), "f"(v2), "r"((int)chunk_lane), "f"(v3) : "memory");
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst + 8 * jj), "f"(u[0]), "f"(u[1]) : "memory");
       }
     } else {
       // ---- coord: this unit's term of trans for rows re, re + 8 (egnn_new.py:100-109), chunk sums
@@ -476,7 +522,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
         float tr[3];
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-          const float d = ex->dir[k][r];
+          const float d = sc->dir[k][r];
           float t;
           if (m == 0) t = a.use_tanh ? (d * tanhf(sv)) * a.coords_range : d * sv;       // coord_diff * tanh(phi) * range
           else t = d * (a.use_tanh ? tanhf(sv) * a.coords_range : sv);                     // coord_cross * (tanh(phi_x) * range)
@@ -495,6 +541,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
         }
       }
     }
+    m = m_next; e0 = e0_next;
   }
 }
 

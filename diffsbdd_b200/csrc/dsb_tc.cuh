@@ -216,21 +216,23 @@ struct WeightStream {
 
 // Per-warpgroup bookkeeping of the asynchronous wgmma groups: every chunk's stage is released (one arrive on empty) once
 // its wgmmas are known to be complete (lane 0 of every warp arrives).  At most one group stays in flight while the next
-// chunk's operand is built.
+// chunk's operand is built (in the edge kernels also across unit boundaries: the next unit's first chunk is built under
+// the last chunk of the current one); the accumulators are read only after drain().
 struct MmaTracker {
   int pend = -1;
+  // after committing chunk g: wait for the previous chunk's group and release its stage
+  __device__ __forceinline__ void release_prev(Control* ctl, int g, bool leader) {
+    wgmma_wait<1>();
+    if (leader && pend >= 0) mbar_arrive(&ctl->empty[pend & 1]);
+    pend = g;
+  }
+  // wait for the last committed group, release its stage; the accumulators are final
   template <int H>
-  __device__ __forceinline__ void after_commit(Control* ctl, float (&d)[H / 2], int g, bool last_of_tile, bool leader) {
-    if (last_of_tile) {
-      wgmma_wait<0>();
-      acc_fence(d);
-      if (leader) { if (pend >= 0) mbar_arrive(&ctl->empty[pend & 1]); mbar_arrive(&ctl->empty[g & 1]); }
-      pend = -1;
-    } else {
-      wgmma_wait<1>();
-      if (leader && pend >= 0) mbar_arrive(&ctl->empty[pend & 1]);
-      pend = g;
-    }
+  __device__ __forceinline__ void drain(Control* ctl, float (&d)[H / 2], bool leader) {
+    wgmma_wait<0>();
+    acc_fence(d);
+    if (leader && pend >= 0) mbar_arrive(&ctl->empty[pend & 1]);
+    pend = -1;
   }
 };
 
