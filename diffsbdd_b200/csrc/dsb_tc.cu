@@ -206,6 +206,23 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
         upk2(x, acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
       }
     }
+    // Residual: every R load is issued before the first store.  R and C may be the same buffer (g3: h += ...), so the
+    // compiler keeps loads and stores in program order; read inside the store loop, each load would wait for the
+    // previous store and the epilogue would pay H / 4 dependent L2 round trips.  Rows past M read row M - 1 (no branch
+    // next to the accumulators) and are not stored.
+    if (g.R) {
+#pragma unroll
+      for (int j = 0; j < H / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = min(m0 + re + 8 * hh, g.M - 1);
+          const f32x2 x = add2(*reinterpret_cast<const float2*>(g.R + (size_t)row * g.ldr + n),
+                               pk2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]));
+          upk2(x, acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+        }
+      }
+    }
     acc_fence(acc);
 #pragma unroll
     for (int j = 0; j < H / 8; ++j) {
@@ -214,9 +231,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
       for (int hh = 0; hh < 2; ++hh) {
         const int row = m0 + re + 8 * hh;
         if (row < g.M) {
-          f32x2 x = pk2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
-          if (g.R) x = add2(*reinterpret_cast<const float2*>(g.R + (size_t)row * g.ldr + n), x);
-          *reinterpret_cast<float2*>(g.C + (size_t)row * g.ldc + n) = x;
+          *reinterpret_cast<float2*>(g.C + (size_t)row * g.ldc + n) = pk2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
           if (g.Z) *reinterpret_cast<float2*>(g.Z + (size_t)row * g.ldz + n) = make_float2(0.f, 0.f);
         }
       }
