@@ -19,7 +19,12 @@ EXPORTED_SYMBOLS = (
     'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_deterministic', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
     'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_ddpm_noise',
     'dsb_ddpm_vlb_terms', 'dsb_last_error', 'dsb_version', 'dsb_dynamics_set_stop_after', 'dsb_workspace_region',
+    'dsb_seeded_normal',
 )
+
+# roles and kinds of dsb_seeded_normal (DSB_RNG_* in include/diffsbdd_b200.h)
+RNG_LIGAND, RNG_POCKET, RNG_JOINT_X, RNG_GRAPH = 0, 1, 2, 3
+RNG_NORMAL, RNG_UNIFORM, RNG_BITS = 0, 1, 2
 
 # workspace regions of dsb_workspace_region (DSB_WS_* in include/diffsbdd_b200.h), in enum order
 WS_REGIONS = ('x_in', 'x_ping', 'x_pong', 'h', 'hT', 'agg', 'P', 'xagg', 'cent', 'deg', 'row_ptr', 'vrow_ptr', 'vmap',
@@ -115,6 +120,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dsb_workspace_region.argtypes = [C.POINTER(DsbConfig), C.c_int, i64, i64, i64, i64, C.c_int, C.POINTER(i64),
                                          C.POINTER(i64)]
     lib.dsb_workspace_region.restype = C.c_int
+    lib.dsb_seeded_normal.argtypes = [vp, i64, i32, i32, vp, vp, vp, vp, i64, i64, i64, vp]
+    lib.dsb_seeded_normal.restype = C.c_int
     _LIB = lib
     return lib
 

@@ -23,7 +23,7 @@ import ctypes as C
 import torch
 import torch.nn.functional as F
 
-from . import _native
+from . import _native, seeded
 from .dynamics import EGNNDynamics
 from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_add, scatter_mean, num_nodes_to_batch_mask
 
@@ -52,7 +52,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         """conditional_model.py:140-160."""
         if fix_noise:
             raise NotImplementedError("fix_noise option isn't implemented yet")
-        eps = self.sample_gaussian(size=(len(lig_mask), self.n_dims + self.atom_nf), device=lig_mask.device)
+        eps = self._lig_noise(lig_mask, self.n_dims + self.atom_nf)
         out_lig = mu_lig + sigma[lig_mask] * eps
         xh_pocket = xh0_pocket.detach().clone()
         out_lig[:, :self.n_dims], xh_pocket[:, :self.n_dims] = self.remove_mean_batch(
@@ -62,7 +62,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def noised_representation(self, xh_lig, xh0_pocket, lig_mask, pocket_mask, gamma_t):
         """conditional_model.py:162-183: z_t ~ q(z_t | x, h) for the ligand; pocket follows the COM shift."""
         alpha_t, sigma_t = self.alpha(gamma_t, xh_lig), self.sigma(gamma_t, xh_lig)
-        eps = self.sample_gaussian(size=(len(lig_mask), self.n_dims + self.atom_nf), device=lig_mask.device)
+        eps = self._lig_noise(lig_mask, self.n_dims + self.atom_nf)
         z_lig = alpha_t[lig_mask] * xh_lig + sigma_t[lig_mask] * eps
         xh_pocket = xh0_pocket.detach().clone()
         z_lig[:, :self.n_dims], xh_pocket[:, :self.n_dims] = self.remove_mean_batch(
@@ -133,14 +133,15 @@ class ConditionalDDPM(EnVariationalDiffusion):
         inp = [self.alpha(gamma_s, s_arr), self.sigma(gamma_s, s_arr), alpha_ts, sigma_ts]
         return t_arr.float().contiguous(), torch.cat([a, c, sg] + inp, dim=1).float().contiguous()
 
-    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps):
+    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, seeds=None):
         """Static buffers + captured graphs for one batch layout.  A cached engine is reused only while everything a
         captured graph bakes in is unchanged: batch layout (mask contents), the native module generation (packed-weight
-        blob), its arithmetic mode and its workspace/status buffers."""
+        blob), its arithmetic mode and its workspace/status buffers, and whether its noise is seeded (the seeds themselves
+        are a static buffer, refreshed on every call)."""
         device = z_lig.device
         dyn: EGNNDynamics = self.dynamics
         dyn._ensure_handle(device)
-        key = (tuple(z_lig.shape), tuple(xh_pocket.shape), n_samples, timesteps, str(device))
+        key = (tuple(z_lig.shape), tuple(xh_pocket.shape), n_samples, timesteps, str(device), seeds is not None)
         st = self._graph_cache.get(key)
         if st is not None:
             same_layout = torch.equal(st['lig_mask'], lig_mask) and torch.equal(st['pocket_mask'], pocket_mask)
@@ -158,8 +159,14 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 coef4=torch.zeros((n_samples, 4), device=device),
                 step=torch.zeros(1, dtype=torch.int64, device=device), t_table=t_table, coef_table=coef_table,
                 lig_mask=lig_mask.clone(), pocket_mask=pocket_mask.clone(), graphs={}, sig=None,
-                n_samples=n_samples, inpaint=None)
+                n_samples=n_samples, inpaint=None, seeded=seeds is not None)
+            if seeds is not None:     # seeds, draw ids of the step's three draws, resampling round u
+                st.update(seeds=torch.empty_like(seeds), draw=torch.zeros(3, dtype=torch.int64, device=device),
+                          u=torch.zeros(1, dtype=torch.int64, device=device))
             self._graph_cache[key] = st
+        if seeds is not None:
+            st['seeds'].copy_(seeds)
+            st['u'].zero_()
         return st
 
     def _captured_step(self, st, kind):
@@ -171,32 +178,58 @@ class ConditionalDDPM(EnVariationalDiffusion):
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
         NL, NP = st['z'].shape[0], st['pocket'].shape[0]
 
+        def draw(out, purpose):
+            seeded.fill(out, _native.RNG_LIGAND, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
+
         def run():
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            if st['seeded']:
+                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
             idx = st['step'].clamp(min=0)
             st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
             row = st['coef_table'].index_select(0, idx)
             st['coef3'].copy_(row[:, :3].expand(n, 3))
             st['coef4'].copy_(row[:, 3:].expand(n, 4))
             eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
-            st['noise'].normal_()
+            if st['seeded']:
+                draw(st['noise'], seeded.PURPOSE_REVERSE)
+            else:
+                st['noise'].normal_()
             _native.check(lib.dsb_ddpm_ligand_update(
                 st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef3'].data_ptr(),
                 lm.data_ptr(), pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf,
                 st['z'].data_ptr(), st['pocket'].data_ptr(), stream))
             if kind != 'reverse':
                 ip = st['inpaint']
-                st['noise1'].normal_()
                 renoise = kind == 'inpaint_renoise'
-                if renoise:
-                    st['noise2'].normal_()
+                if st['seeded']:
+                    draw(st['noise1'], seeded.PURPOSE_KNOWN)
+                    if renoise:
+                        draw(st['noise2'], seeded.PURPOSE_RENOISE)
+                else:
+                    st['noise1'].normal_()
+                    if renoise:
+                        st['noise2'].normal_()
                 _native.check(lib.dsb_ddpm_inpaint_update(
                     st['z'].data_ptr(), st['pocket'].data_ptr(), ip['known'].data_ptr(), ip['com0'].data_ptr(),
                     ip['fixed'].data_ptr(), st['noise1'].data_ptr(), st['noise2'].data_ptr() if renoise else None,
                     st['coef4'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, stream))
             if kind != 'inpaint_renoise':
                 st['step'].sub_(1)
+            if st['seeded'] and kind != 'reverse':
+                if kind == 'inpaint_renoise':
+                    st['u'].add_(1)
+                else:
+                    st['u'].zero_()
         return run
+
+    @staticmethod
+    def _start(st, z_lig, xh_pocket, first_s):
+        """Loads the static state a run of captured steps starts from: z, pocket, step and (seeded) the resampling round
+        u = 0.  A warm-up run advances u like any other, so capture resets it here as well."""
+        st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
+        if st['seeded']:
+            st['u'].zero_()
 
     def _graph(self, st, kind, z_lig, xh_pocket, first_s):
         """Captured CUDA graph of ``kind`` (captured on first use; capture leaves the static state as it found it)."""
@@ -208,7 +241,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         run = self._captured_step(st, kind)
 
         def reset():
-            st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
+            self._start(st, z_lig, xh_pocket, first_s)
 
         # warm-up on a side stream (allocator + plan caches + workspace), restoring RNG and state afterwards.  It runs on the
         # real inputs: the static buffers start uninitialised, and a NaN left there by an earlier allocation would set the
@@ -236,12 +269,12 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def _graphed_reverse_steps(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, first_s, n_steps, timesteps):
         """Runs reverse steps s = first_s, first_s-1, ..., first_s-n_steps+1 by replaying one captured step."""
         dyn: EGNNDynamics = self.dynamics
-        st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps)
+        st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, self._seeds())
         prev_defer = dyn.defer_status_check
         dyn.defer_status_check = True
         try:
             g = self._graph(st, 'reverse', z_lig, xh_pocket, first_s)
-            st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
+            self._start(st, z_lig, xh_pocket, first_s)
             for _ in range(n_steps):
                 g.replay()
         finally:
@@ -255,7 +288,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         denoiser + fused reverse update + fused RePaint iteration (dsb_ddpm_inpaint_update); no torch op and no host
         sync inside the loop."""
         dyn: EGNNDynamics = self.dynamics
-        st = self._engine(z_lig, xh_pocket, lmask, pmask, n_samples, timesteps)
+        st = self._engine(z_lig, xh_pocket, lmask, pmask, n_samples, timesteps, self._seeds())
         if st['inpaint'] is None:       # static buffers the captured RePaint iteration reads
             st['inpaint'] = dict(known=torch.empty_like(z_lig), com0=torch.empty_like(com_pocket_0, dtype=torch.float32),
                                  fixed=torch.empty(z_lig.shape[0], dtype=torch.float32, device=z_lig.device))
@@ -267,7 +300,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         try:
             g_last = self._graph(st, 'inpaint_last', z_lig, xh_pocket, s0)
             g_re = self._graph(st, 'inpaint_renoise', z_lig, xh_pocket, s0) if resamplings > 1 else None
-            st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(s0)
+            self._start(st, z_lig, xh_pocket, s0)
             for s in reversed(range(0, timesteps)):
                 for _ in range(resamplings - 1):
                     g_re.replay()
@@ -283,22 +316,32 @@ class ConditionalDDPM(EnVariationalDiffusion):
     # ---- public samplers ------------------------------------------------------------------------------------
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None):
-        """conditional_model.py:479-555."""
+    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None):
+        """conditional_model.py:479-555.  ``seeds``: one int64 per sample (seeded.py); every draw then comes from the
+        sample's own seed instead of torch's global generator."""
         timesteps = self.T if timesteps is None else timesteps
         assert 0 < return_frames <= timesteps
         assert timesteps % return_frames == 0
         n_samples = len(pocket['size'])
         device = pocket['x'].device
+        seeds = seeded.as_seeds(seeds, n_samples, device)
+        lig_mask = num_nodes_to_batch_mask(n_samples, num_nodes_lig, device)
+        with self._seeded(seeds, lig_mask, pocket['mask']):
+            return self._sample_given_pocket(pocket, lig_mask, n_samples, return_frames, timesteps)
+
+    def _sample_given_pocket(self, pocket, lig_mask, n_samples, return_frames, timesteps):
+        if self._rng is not None:
+            seeded.check_schedule(timesteps)
+        device = pocket['x'].device
         _, pocket = self.normalize(pocket=pocket)
         xh0_pocket = torch.cat([pocket['x'], pocket['one_hot']], dim=1)
-        lig_mask = num_nodes_to_batch_mask(n_samples, num_nodes_lig, device)
 
         # ligand prior centred on the pocket COM (conditional_model.py:501-510)
         mu_lig_x = scatter_mean(pocket['x'], pocket['mask'], dim=0)
         mu_lig_h = torch.zeros((n_samples, self.atom_nf), device=device)
         mu_lig = torch.cat((mu_lig_x, mu_lig_h), dim=1)[lig_mask]
         sigma = torch.ones_like(pocket['size']).unsqueeze(1)
+        self._draw_at(seeded.STAGE_PRIOR)
         z_lig, xh_pocket = self.sample_normal_zero_com(mu_lig, xh0_pocket, sigma, lig_mask, pocket['mask'])
         self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
 
@@ -320,27 +363,36 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
                 t_array = (s_array + 1) / timesteps
                 s_array = s_array / timesteps
+                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
                 z_lig, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, xh_pocket, lig_mask, pocket['mask'])
                 if (s * return_frames) % timesteps == 0:
                     idx = (s * return_frames) // timesteps
                     out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
 
+        self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples)
         self.assert_mean_zero_with_mask(x_lig, lig_mask)
         if return_frames == 1:                          # conditional_model.py:540-547
-            max_cog = scatter_add(x_lig, lig_mask, dim=0).abs().max().item()
-            if max_cog > 5e-2:
-                print(f'Warning CoG drift with error {max_cog:.3f}. Projecting the positions down.')
-                x_lig, x_pocket = self.remove_mean_batch(x_lig, x_pocket, lig_mask, pocket['mask'])
+            x_lig, x_pocket = self._project_cog_drift(
+                x_lig, x_pocket, lig_mask, lambda: self.remove_mean_batch(x_lig, x_pocket, lig_mask, pocket['mask']),
+                pocket['mask'])
         out_lig[0] = torch.cat([x_lig, h_lig], dim=1)
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lig_mask, pocket['mask']
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def inpaint(self, ligand, pocket, lig_fixed, resamplings=1, return_frames=1, timesteps=None, center='ligand'):
-        """conditional_model.py:558-686: RePaint-style conditional generation with fixed ligand atoms."""
+    def inpaint(self, ligand, pocket, lig_fixed, resamplings=1, return_frames=1, timesteps=None, center='ligand', seeds=None):
+        """conditional_model.py:558-686: RePaint-style conditional generation with fixed ligand atoms.  ``seeds``: as
+        sample_given_pocket."""
+        seeds = seeded.as_seeds(seeds, len(ligand['size']), pocket['x'].device)
+        with self._seeded(seeds, ligand['mask'], pocket['mask']):
+            return self._inpaint(ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center)
+
+    def _inpaint(self, ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center):
         timesteps = self.T if timesteps is None else timesteps
+        if self._rng is not None:
+            seeded.check_schedule(timesteps, resamplings)
         assert 0 < return_frames <= timesteps
         assert timesteps % return_frames == 0
         if len(lig_fixed.size()) == 1:
@@ -363,6 +415,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
         mu_lig = torch.cat((mean_known, torch.zeros((n_samples, self.atom_nf), device=device)), dim=1)[lmask]
         sigma = torch.ones_like(pocket['size']).unsqueeze(1)
+        self._draw_at(seeded.STAGE_PRIOR)
         z_lig, xh_pocket = self.sample_normal_zero_com(mu_lig, xh0_pocket, sigma, lmask, pmask)
 
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
@@ -382,11 +435,13 @@ class ConditionalDDPM(EnVariationalDiffusion):
                     gamma_t, gamma_s = self.gamma(t_array), self.gamma(s_array)
 
                     # denoise the whole ligand one step (unknown part)
+                    self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
                     z_unknown, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, xh_pocket, lmask, pmask)
 
                     # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
                     com_pocket = scatter_mean(xh_pocket[:, :nd], pmask, dim=0)
                     xh_ligand[:, :nd] = ligand['x'] + (com_pocket - com_pocket_0)[lmask]
+                    self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_KNOWN)
                     z_known, xh_pocket, _ = self.noised_representation(xh_ligand, xh_pocket, lmask, pmask, gamma_s)
 
                     # align COM of the fixed atoms: noised -> denoised (conditional_model.py:645-656)
@@ -398,11 +453,13 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
                     z_lig = z_known * lig_fixed + z_unknown * (1 - lig_fixed)
                     if u < resamplings - 1:
+                        self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_RENOISE)
                         z_lig, xh_pocket = self.sample_p_zt_given_zs(z_lig, xh_pocket, lmask, pmask, gamma_t, gamma_s)
                     if u == resamplings - 1 and (s * return_frames) % timesteps == 0:
                         idx = (s * return_frames) // timesteps
                         out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
 
+        self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, xh_pocket, lmask, pmask, n_samples)
         out_lig[0] = torch.cat([x_lig, h_lig], dim=1)
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
@@ -520,9 +577,18 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def diversify(self, ligand, pocket, noising_steps):
-        """conditional_model.py:364-409: partially noise given ligands, then denoise them again."""
+    def diversify(self, ligand, pocket, noising_steps, seeds=None):
+        """conditional_model.py:364-409: partially noise given ligands, then denoise them again.  ``seeds``: as
+        sample_given_pocket."""
+        seeds = seeded.as_seeds(seeds, len(pocket['size']), pocket['x'].device)
+        with self._seeded(seeds, ligand['mask'], pocket['mask']):
+            return self._diversify(ligand, pocket, noising_steps)
+
+    def _diversify(self, ligand, pocket, noising_steps):
+        if self._rng is not None:
+            seeded.check_schedule(self.T)
         ligand, pocket = self.normalize(ligand, pocket)
+        self._draw_at(seeded.STAGE_PARTIAL)
         z_lig, xh_pocket, _ = self.partially_noised_ligand(ligand, pocket, noising_steps)
         timesteps = self.T
         n_samples = len(pocket['size'])
@@ -536,8 +602,10 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
                 t_array = (s_array + 1) / timesteps
                 s_array = s_array / timesteps
+                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
                 z_lig, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig.detach(), xh_pocket.detach(),
                                                              lig_mask, pocket['mask'])
+        self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples)
         self.assert_mean_zero_with_mask(x_lig, lig_mask)
         return torch.cat([x_lig, h_lig], dim=1), torch.cat([x_pocket, h_pocket], dim=1), lig_mask, pocket['mask']
@@ -574,7 +642,7 @@ class SimpleConditionalDDPM(ConditionalDDPM):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None):
+    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None):
         pocket_com = scatter_mean(pocket['x'], pocket['mask'], dim=0)
         pocket['x'] = pocket['x'] - pocket_com[pocket['mask']]
-        return super().sample_given_pocket(pocket, num_nodes_lig, return_frames, timesteps)
+        return super().sample_given_pocket(pocket, num_nodes_lig, return_frames, timesteps, seeds)

@@ -651,6 +651,68 @@ __global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
   }
 }
 
+// ---- seeded per-graph random numbers (dsb_seeded_normal; the contract is in include/diffsbdd_b200.h) -------------------
+// Philox4x32-10 (Salmon et al., SC'11): 10 rounds, the key bumped by the Weyl constants between rounds.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// (0, 1]: (w + 1/2) 2^-32 with w rounded to fp32 first; never 0, so log() is finite
+__device__ __forceinline__ float rng_uniform(uint32_t w) { return fmaf((float)w, 0x1p-32f, 0x1p-33f); }
+
+// One thread per (row, group of 4 columns).  The row's graph and its index within the graph come from the sorted masks.
+__global__ void __launch_bounds__(128) seeded_rng_kernel(float* __restrict__ out, int rows, int cols, int role, int kind,
+                                                          const int64_t* __restrict__ seeds, const int64_t* __restrict__ draw_id,
+                                                          const int64_t* __restrict__ mask_atoms,
+                                                          const int64_t* __restrict__ mask_res, int NL, int NP) {
+  const int groups = (cols + 3) >> 2;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)rows * groups) return;
+  const int r = (int)(i / groups), grp = (int)(i - (int64_t)r * groups);
+  int64_t g;
+  int local;
+  if (role == DSB_RNG_GRAPH) {
+    g = r; local = 0;
+  } else if (role == DSB_RNG_POCKET || (role == DSB_RNG_JOINT_X && r >= NL)) {
+    const int p = role == DSB_RNG_POCKET ? r : r - NL;
+    g = mask_res[p];
+    local = p - lb64(mask_res, NP, g);
+    if (role == DSB_RNG_JOINT_X) local += lb64(mask_atoms, NL, g + 1) - lb64(mask_atoms, NL, g);   // after the graph's ligand rows
+  } else {
+    g = mask_atoms[r];
+    local = r - lb64(mask_atoms, NL, g);
+  }
+  const uint64_t seed = (uint64_t)seeds[g], draw = (uint64_t)draw_id[0];
+  const uint4 w = philox4x32_10(make_uint4((uint32_t)grp, (uint32_t)local, (uint32_t)role | ((uint32_t)(draw >> 32) << 4),
+                                           (uint32_t)draw),
+                                (uint32_t)seed, (uint32_t)(seed >> 32));
+  float v[4];
+  if (kind == DSB_RNG_NORMAL) {                 // Box-Muller on the pairs (w.x, w.y) and (w.z, w.w)
+    float s, c;
+    const float r0 = sqrtf(-2.f * logf(rng_uniform(w.x)));
+    sincospif(2.f * ((float)w.y * 0x1p-32f), &s, &c);
+    v[0] = r0 * c; v[1] = r0 * s;
+    const float r1 = sqrtf(-2.f * logf(rng_uniform(w.z)));
+    sincospif(2.f * ((float)w.w * 0x1p-32f), &s, &c);
+    v[2] = r1 * c; v[3] = r1 * s;
+  } else if (kind == DSB_RNG_UNIFORM) {
+    v[0] = rng_uniform(w.x); v[1] = rng_uniform(w.y); v[2] = rng_uniform(w.z); v[3] = rng_uniform(w.w);
+  } else {
+    v[0] = __uint_as_float(w.x); v[1] = __uint_as_float(w.y); v[2] = __uint_as_float(w.z); v[3] = __uint_as_float(w.w);
+  }
+  float* const o = out + (size_t)r * cols + 4 * grp;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (4 * grp + k < cols) o[k] = v[k];
+}
+
 // ---- evaluation-mode variational bound (ConditionalDDPM / EnVariationalDiffusion.forward, eval branch) ----------------
 // z = alpha[g] xh + sigma[g] eps for ligand rows and (optional) pocket rows: q(z_t | x, h) of the joint model
 // (en_diffusion.py:302-317, eps.x already COM-free) and of SimpleConditionalDDPM (no COM projection, :702-735).
@@ -1174,6 +1236,30 @@ int dsb_ddpm_vlb_terms(const float* xh0_lig, const float* z_t_lig, const float* 
       xh0_lig, z_t_lig, eps_t_lig, net_t_lig, z_0_lig, eps_0_lig, net_0_lig, xh0_pocket, eps_t_pocket, net_t_pocket, z_0_pocket,
       eps_0_pocket, net_0_pocket, coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, norm_value_h,
       norm_bias_h, vnode_idx, terms, xh_lig_hat);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_seeded_normal(float* out, int64_t cols, int32_t role, int32_t kind, const int64_t* seeds, const int64_t* draw_id,
+                      const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues,
+                      int64_t n_graphs, void* stream) {
+  if (role < DSB_RNG_LIGAND || role > DSB_RNG_GRAPH || kind < DSB_RNG_NORMAL || kind > DSB_RNG_BITS || cols <= 0 ||
+      cols > (1 << 18)) {
+    set_error("dsb_seeded_normal: bad role=%d kind=%d cols=%lld", role, kind, (long long)cols);
+    return DSB_ERR_INVALID_ARGUMENT;
+  }
+  if (int rc = check_sizes(n_atoms, n_residues, n_graphs, 0)) return rc;
+  const int64_t rows = role == DSB_RNG_LIGAND ? n_atoms : role == DSB_RNG_POCKET ? n_residues
+                     : role == DSB_RNG_JOINT_X ? n_atoms + n_residues : n_graphs;
+  if (rows <= 0) return 0;
+  const bool need_lig = role == DSB_RNG_LIGAND || (role == DSB_RNG_JOINT_X && n_atoms > 0);
+  const bool need_poc = role == DSB_RNG_POCKET || (role == DSB_RNG_JOINT_X && n_residues > 0);
+  if (!out || !seeds || !draw_id || (need_lig && !mask_atoms) || (need_poc && !mask_residues)) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  const int64_t threads = rows * ((cols + 3) / 4);
+  seeded_rng_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      out, (int)rows, (int)cols, role, kind, seeds, draw_id, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues);
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }

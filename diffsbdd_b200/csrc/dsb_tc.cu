@@ -475,6 +475,30 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
     const float* b2 = ex->vec[m] + 2 * H;
     const f32x2 ip = pk2(a.inv_scale[m], a.inv_scale[m]);
     float s_lo = 0.f, s_hi = 0.f;
+    if constexpr (DET) {
+      // Batch-invariant grouping: the shared-reciprocal SiLU takes column groups jj and jj + 1 of ONE row (re, then re + 8),
+      // so an edge's messages depend on that edge alone, not on the edge 8 rows away (which changes with the batch layout).
+      // Same number of SiLU calls as below; the row sums s keep their column order.
+      static_assert((H / 8) % 2 == 0, "DET epilogue pairs column groups");
+#pragma unroll
+      for (int jj = 0; jj < H / 8; jj += 2) {
+        const int c = 8 * jj + 2 * (lane & 3);
+        const f32x2 b0 = *reinterpret_cast<const float2*>(b2 + c), b1 = *reinterpret_cast<const float2*>(b2 + c + 8);
+        const float2 w0 = *reinterpret_cast<const float2*>(ex->wa + c), w1 = *reinterpret_cast<const float2*>(ex->wa + c + 8);
+        f32x2 lo0 = pk2(acc[4 * jj], acc[4 * jj + 1]), lo1 = pk2(acc[4 * jj + 4], acc[4 * jj + 5]);
+        f32x2 hi0 = pk2(acc[4 * jj + 2], acc[4 * jj + 3]), hi1 = pk2(acc[4 * jj + 6], acc[4 * jj + 7]);
+        lo0 = F16 ? fma2(lo0, ip, b0) : add2(lo0, b0); lo1 = F16 ? fma2(lo1, ip, b1) : add2(lo1, b1);
+        hi0 = F16 ? fma2(hi0, ip, b0) : add2(hi0, b0); hi1 = F16 ? fma2(hi1, ip, b1) : add2(hi1, b1);
+        silu_pair<(DSB_SILU_PAIR & 2) != 0, (DSB_SILU_QUAD & 2) != 0>(lo0, lo1);
+        silu_pair<(DSB_SILU_PAIR & 2) != 0, (DSB_SILU_QUAD & 2) != 0>(hi0, hi1);
+        upk2(lo0, acc[4 * jj], acc[4 * jj + 1]); upk2(lo1, acc[4 * jj + 4], acc[4 * jj + 5]);
+        upk2(hi0, acc[4 * jj + 2], acc[4 * jj + 3]); upk2(hi1, acc[4 * jj + 6], acc[4 * jj + 7]);
+        s_lo = fmaf(lo0.y, w0.y, fmaf(lo0.x, w0.x, s_lo));
+        s_lo = fmaf(lo1.y, w1.y, fmaf(lo1.x, w1.x, s_lo));
+        s_hi = fmaf(hi0.y, w0.y, fmaf(hi0.x, w0.x, s_hi));
+        s_hi = fmaf(hi1.y, w1.y, fmaf(hi1.x, w1.x, s_hi));
+      }
+    } else {
 #pragma unroll
     for (int jj = 0; jj < H / 8; ++jj) {
       const int c = 8 * jj + 2 * (lane & 3);
@@ -487,6 +511,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
       upk2(lo, acc[4 * jj], acc[4 * jj + 1]); upk2(hi, acc[4 * jj + 2], acc[4 * jj + 3]);
       s_lo = fmaf(lo.y, ww.y, fmaf(lo.x, ww.x, s_lo));
       s_hi = fmaf(hi.y, ww.y, fmaf(hi.x, ww.x, s_hi));
+    }
     }
     s_lo += __shfl_xor_sync(0xffffffffu, s_lo, 1); s_lo += __shfl_xor_sync(0xffffffffu, s_lo, 2);
     s_hi += __shfl_xor_sync(0xffffffffu, s_hi, 1); s_hi += __shfl_xor_sync(0xffffffffu, s_hi, 2);

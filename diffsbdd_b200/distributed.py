@@ -30,13 +30,24 @@ def shard_pocket(pocket: Dict[str, torch.Tensor], lo: int, hi: int) -> Dict[str,
 
 
 @torch.no_grad()
+def shard_seeds(seeds, lo: int, hi: int) -> torch.Tensor:
+    """This rank's slice [lo, hi) of the whole job's per-sample seeds, as an int64 tensor."""
+    seeds = seeds if isinstance(seeds, torch.Tensor) else torch.as_tensor(seeds, dtype=torch.int64)
+    return seeds[lo:hi]
+
+
+@torch.no_grad()
 def sample_given_pocket_sharded(ddpm, pocket: Dict[str, torch.Tensor], num_nodes_lig: torch.Tensor, base_seed: int = 0,
-                                timesteps=None, group=None):
+                                timesteps=None, group=None, seeds=None):
     """Runs ``ddpm.sample_given_pocket`` on this rank's shard of the pockets and gathers the ligands of all ranks.
 
     ``pocket``/``num_nodes_lig`` describe the WHOLE job on every rank (device tensors of this rank).  Returns
     ``(xh_lig_all, lig_sizes_all)`` — identical on every rank, ordered by global pocket index — plus this rank's own
     ``(xh_lig, xh_pocket, lig_mask, pocket_mask)`` tuple.
+
+    ``seeds`` (one int64 per pocket of the whole job): rank r samples its pockets with ``seeds[lo:hi]`` and ``base_seed`` is
+    ignored, so in deterministic mode the gathered ligands are the same for any number of ranks.  Without ``seeds`` every
+    rank draws from torch's generator seeded with ``base_seed + rank``.
     """
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
@@ -44,11 +55,18 @@ def sample_given_pocket_sharded(ddpm, pocket: Dict[str, torch.Tensor], num_nodes
     lo, hi = shard_bounds(n, world, rank)
     dev = pocket['x'].device
     gen_state = torch.random.get_rng_state()
-    torch.manual_seed(base_seed + rank)
-    if dev.type == 'cuda':
-        torch.cuda.manual_seed(base_seed + rank)
+    if seeds is not None:
+        if len(seeds) != n:
+            raise ValueError(f'seeds must hold one value per pocket of the whole job: {n} expected, got {len(seeds)}')
+        local_seeds = shard_seeds(seeds, lo, hi)
+    else:
+        local_seeds = None
+        torch.manual_seed(base_seed + rank)
+        if dev.type == 'cuda':
+            torch.cuda.manual_seed(base_seed + rank)
     if hi > lo:
-        local = ddpm.sample_given_pocket(shard_pocket(pocket, lo, hi), num_nodes_lig[lo:hi], timesteps=timesteps)
+        local = ddpm.sample_given_pocket(shard_pocket(pocket, lo, hi), num_nodes_lig[lo:hi], timesteps=timesteps,
+                                         **({} if local_seeds is None else {'seeds': local_seeds}))
     else:
         width = ddpm.n_dims + ddpm.atom_nf
         local = (torch.zeros((0, width), device=dev), torch.zeros((0, ddpm.n_dims + ddpm.residue_nf), device=dev),

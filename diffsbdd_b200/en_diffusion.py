@@ -215,6 +215,7 @@ class EnVariationalDiffusion(nn.Module):
     ``dsb_ddpm_joint_inpaint_update``); 'eager' keeps the reference-order Python loop (same torch ops, same RNG calls)."""
 
     loop_engine = 'auto'
+    _rng = None              # seeded.SeededDraws of the running seeded sampler call (None: torch's global generator)
 
     def __init__(self, dynamics: nn.Module, atom_nf: int, residue_nf: int, n_dims: int, size_histogram: Dict,
                  timesteps: int = 1000, parametrization='eps', noise_schedule='learned', noise_precision=1e-4,
@@ -311,6 +312,50 @@ class EnVariationalDiffusion(nn.Module):
     def sample_gaussian(size, device):
         return torch.randn(size, device=device)
 
+    # ---- seeded draws (seeded.py): active inside a sampler call that was given seeds= -----------------------------
+    @contextlib.contextmanager
+    def _seeded(self, seeds, lig_mask, pocket_mask):
+        from .seeded import SeededDraws
+        prev = self._rng
+        self._rng = None if seeds is None else SeededDraws(seeds, lig_mask, pocket_mask)
+        try:
+            yield
+        finally:
+            self._rng = prev
+
+    def _draw_at(self, stage, s=0, u=0, purpose=0):
+        """Sets the draw id of the next seeded draws (no-op without seeds)."""
+        if self._rng is not None:
+            self._rng.at(stage, s, u, purpose)
+
+    def _seeds(self):
+        return None if self._rng is None else self._rng.seeds
+
+    def _lig_noise(self, lig_mask, cols):
+        if self._rng is None:
+            return self.sample_gaussian(size=(len(lig_mask), cols), device=lig_mask.device)
+        from ._native import RNG_LIGAND
+        return self._rng.normal(RNG_LIGAND, cols)
+
+    def _project_cog_drift(self, x_lig, x_pocket, lig_mask, project, pocket_mask, x_all=None, all_mask=None):
+        """The final CoG-drift projection of the samplers (conditional_model.py:540-547, en_diffusion.py:637-646): without
+        seeds, as the reference, every graph is projected when any graph's CoG exceeds 5e-2.  With seeds only the graphs whose
+        own CoG exceeds it are projected, so that a graph's result does not depend on its batch (the one deviation from the
+        reference, and only with seeds).  ``project()`` returns the projected (x_lig, x_pocket)."""
+        cog = scatter_add(x_lig if x_all is None else x_all, lig_mask if all_mask is None else all_mask, dim=0).abs()
+        if self._rng is None:
+            max_cog = cog.max().item()
+            if max_cog > 5e-2:
+                print(f'Warning CoG drift with error {max_cog:.3f}. Projecting the positions down.')
+                return project()
+            return x_lig, x_pocket
+        drift = cog.amax(dim=1) > 5e-2
+        if not bool(drift.any()):
+            return x_lig, x_pocket
+        print(f'Warning CoG drift in {int(drift.sum())} graph(s), max error {cog.max().item():.3f}. Projecting those graphs.')
+        pl, pp = project()
+        return (torch.where(drift[lig_mask].unsqueeze(1), pl, x_lig), torch.where(drift[pocket_mask].unsqueeze(1), pp, x_pocket))
+
     @staticmethod
     def sum_except_batch(x, indices):
         return scatter_add(x.sum(-1), indices, dim=0)
@@ -329,6 +374,11 @@ class EnVariationalDiffusion(nn.Module):
     def sample_combined_position_feature_noise(self, lig_indices, pocket_indices):
         """en_diffusion.py:559-578: COM-free x noise over ligand+pocket, plain h noise."""
         nl, npk = len(lig_indices), len(pocket_indices)
+        if self._rng is not None:
+            from . import _native
+            zx = self.remove_mean_batch(self._rng.normal(_native.RNG_JOINT_X, self.n_dims), torch.cat((lig_indices, pocket_indices)))
+            return (torch.cat([zx[:nl], self._rng.normal(_native.RNG_LIGAND, self.atom_nf)], dim=1),
+                    torch.cat([zx[nl:], self._rng.normal(_native.RNG_POCKET, self.residue_nf)], dim=1))
         zx = self.sample_center_gravity_zero_gaussian_batch((nl + npk, self.n_dims), lig_indices, pocket_indices)
         z_lig = torch.cat([zx[:nl], self.sample_gaussian((nl, self.atom_nf), lig_indices.device)], dim=1)
         z_pocket = torch.cat([zx[nl:], self.sample_gaussian((npk, self.residue_nf), pocket_indices.device)], dim=1)
@@ -425,7 +475,8 @@ class EnVariationalDiffusion(nn.Module):
         dyn = self.dynamics
         device = z_lig.device
         dyn._ensure_handle(device)
-        key = (tuple(z_lig.shape), tuple(z_pocket.shape), n_samples, timesteps, jump_length, str(device))
+        seeds = self._seeds()
+        key = (tuple(z_lig.shape), tuple(z_pocket.shape), n_samples, timesteps, jump_length, str(device), seeds is not None)
         st = self._joint_cache.get(key)
         if st is not None:
             same = torch.equal(st['lig_mask'], lig_mask) and torch.equal(st['pocket_mask'], pocket_mask)
@@ -441,32 +492,47 @@ class EnVariationalDiffusion(nn.Module):
                       t=torch.zeros((n_samples, 1), device=device), coef3=torch.zeros((n_samples, 3), device=device),
                       coef4=torch.zeros((n_samples, 4), device=device), step=torch.zeros(1, dtype=torch.int64, device=device),
                       t_table=t_table, coef_table=coef_table, lig_mask=lig_mask.clone(), pocket_mask=pocket_mask.clone(),
-                      graphs={}, sig=None, n_samples=n_samples, jump=jump_length, known=None)
+                      graphs={}, sig=None, n_samples=n_samples, jump=jump_length, known=None, seeded=seeds is not None)
+            if seeds is not None:     # seeds, draw ids of the step's three draws, jumps back so far u
+                st.update(seeds=torch.empty_like(seeds), draw=torch.zeros(3, dtype=torch.int64, device=device),
+                          u=torch.zeros(1, dtype=torch.int64, device=device))
             self._joint_cache[key] = st
+        if seeds is not None:
+            st['seeds'].copy_(seeds)
+            st['u'].zero_()
         return st
 
     def _joint_step(self, st, kind):
         """kind: 'reverse' (sample: one joint reverse step, step -= 1) | 'inpaint' (noised known part + reverse step + blend,
         step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1)."""
         import ctypes as C
-        from . import _native
+        from . import _native, seeded
         dyn, lib = self.dynamics, _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
         NL, NP = st['zl'].shape[0], st['zp'].shape[0]
         ptr = lambda x: x.data_ptr()
+        roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
+
+        def draw(bufs, purpose):
+            if st['seeded']:
+                for x, role in zip(bufs, roles):
+                    seeded.fill(x, role, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
+            else:
+                for x in bufs:
+                    x.normal_()
 
         def run():
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            if st['seeded']:
+                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
             if kind != 'reverse':                       # eager order: noised_representation draws first (en_diffusion.py:741)
-                for x in st['n_known']:
-                    x.normal_()
+                draw(st['n_known'], seeded.PURPOSE_KNOWN)
             row = st['coef_table'].index_select(0, st['step'].clamp(min=0))
             st['t'].copy_(st['t_table'].index_select(0, st['step'].clamp(min=0)).expand(n, 1))
             st['coef3'].copy_(row[:, :3].expand(n, 3))
             st['coef4'].copy_(row[:, 3:].expand(n, 4))
             eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
-            for x in st['n_rev']:
-                x.normal_()
+            draw(st['n_rev'], seeded.PURPOSE_REVERSE)
             nx, nhl, nhp = st['n_rev']
             _native.check(lib.dsb_ddpm_joint_update(
                 ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef3']),
@@ -475,8 +541,7 @@ class EnVariationalDiffusion(nn.Module):
                 kn = st['known']
                 jump = kind == 'inpaint_jump'
                 if jump:
-                    for x in st['n_jump']:
-                        x.normal_()
+                    draw(st['n_jump'], seeded.PURPOSE_RENOISE)
                 j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
                 _native.check(lib.dsb_ddpm_joint_inpaint_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
@@ -484,9 +549,19 @@ class EnVariationalDiffusion(nn.Module):
                     self.atom_nf, self.residue_nf, stream))
             if kind == 'inpaint_jump':
                 st['step'].add_(st['jump'] - 1)
+                if st['seeded']:
+                    st['u'].add_(1)
             else:
                 st['step'].sub_(1)
         return run
+
+    @staticmethod
+    def _joint_start(st, z_lig, z_pocket, first_s):
+        """Loads the static state a run of captured joint steps starts from: z, step and (seeded) the jump count u = 0.  A
+        warm-up run advances u like any other, so capture resets it here as well."""
+        st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
+        if st['seeded']:
+            st['u'].zero_()
 
     def _joint_graph(self, st, kind, z_lig, z_pocket, first_s):
         g = st['graphs'].get(kind)
@@ -496,7 +571,7 @@ class EnVariationalDiffusion(nn.Module):
         run = self._joint_step(st, kind)
 
         def reset():
-            st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
+            self._joint_start(st, z_lig, z_pocket, first_s)
 
         rng = torch.cuda.get_rng_state(device)
         side = torch.cuda.Stream(device=device)
@@ -526,7 +601,7 @@ class EnVariationalDiffusion(nn.Module):
         prev_defer, dyn.defer_status_check = dyn.defer_status_check, True
         try:
             g = self._joint_graph(st, 'reverse', z_lig, z_pocket, first_s)
-            st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
+            self._joint_start(st, z_lig, z_pocket, first_s)
             for _ in range(n_steps):
                 g.replay()
         finally:
@@ -536,13 +611,24 @@ class EnVariationalDiffusion(nn.Module):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu'):
-        """en_diffusion.py:581-651: unconditional joint sampling of ligand and pocket."""
-        timesteps = self.T if timesteps is None else timesteps
-        assert 0 < return_frames <= timesteps and timesteps % return_frames == 0
+    def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu', seeds=None):
+        """en_diffusion.py:581-651: unconditional joint sampling of ligand and pocket.  ``seeds``: one int64 per sample
+        (seeded.py); every draw then comes from the sample's own seed instead of torch's global generator."""
+        from . import seeded
+        seeds = seeded.as_seeds(seeds, n_samples, device)
         lig_mask = num_nodes_to_batch_mask(n_samples, num_nodes_lig, device)
         pocket_mask = num_nodes_to_batch_mask(n_samples, num_nodes_pocket, device)
+        with self._seeded(seeds, lig_mask, pocket_mask):
+            return self._sample(n_samples, lig_mask, pocket_mask, return_frames, timesteps)
+
+    def _sample(self, n_samples, lig_mask, pocket_mask, return_frames, timesteps):
+        from . import seeded
+        timesteps = self.T if timesteps is None else timesteps
+        assert 0 < return_frames <= timesteps and timesteps % return_frames == 0
+        if self._rng is not None:
+            seeded.check_schedule(timesteps)
         combined_mask = torch.cat((lig_mask, pocket_mask))
+        self._draw_at(seeded.STAGE_PRIOR)
         z_lig, z_pocket = self.sample_combined_position_feature_noise(lig_mask, pocket_mask)
         self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
@@ -562,18 +648,16 @@ class EnVariationalDiffusion(nn.Module):
                 s_arr = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
                 t_arr = (s_arr + 1) / timesteps
                 s_arr = s_arr / timesteps
+                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
                 z_lig, z_pocket = self.sample_p_zs_given_zt(s_arr, t_arr, z_lig, z_pocket, lig_mask, pocket_mask)
                 if (s * return_frames) % timesteps == 0:
                     idx = (s * return_frames) // timesteps
                     out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
+        self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, z_pocket, lig_mask, pocket_mask, n_samples)
         self.assert_mean_zero_with_mask(torch.cat((x_lig, x_pocket), dim=0), combined_mask)
         if return_frames == 1:
-            max_cog = scatter_add(torch.cat((x_lig, x_pocket)), combined_mask, dim=0).abs().max().item()
-            if max_cog > 5e-2:
-                print(f'Warning CoG drift with error {max_cog:.3f}. Projecting the positions down.')
-                xc = self.remove_mean_batch(torch.cat((x_lig, x_pocket)), combined_mask)
-                x_lig, x_pocket = xc[:len(x_lig)], xc[len(x_lig):]
+            x_lig, x_pocket = self._project_joint_cog_drift(x_lig, x_pocket, lig_mask, pocket_mask)
         out_lig[0] = torch.cat([x_lig, h_lig], dim=1)
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lig_mask, pocket_mask
@@ -595,6 +679,15 @@ class EnVariationalDiffusion(nn.Module):
             done += step
         return blocks[::-1]
 
+    def _project_joint_cog_drift(self, x_lig, x_pocket, lig_mask, pocket_mask):
+        combined_mask = torch.cat((lig_mask, pocket_mask))
+        xc = torch.cat((x_lig, x_pocket))
+
+        def project():
+            xp = self.remove_mean_batch(xc, combined_mask)
+            return xp[:len(x_lig)], xp[len(x_lig):]
+        return self._project_cog_drift(x_lig, x_pocket, lig_mask, project, pocket_mask, xc, combined_mask)
+
     def _fixed_com(self, x_lig, x_pocket, lig_sel, pocket_sel, lig_mask, pocket_mask):
         """COM of the fixed ligand+pocket nodes per graph."""
         return scatter_mean(torch.cat((x_lig[lig_sel], x_pocket[pocket_sel])),
@@ -603,9 +696,18 @@ class EnVariationalDiffusion(nn.Module):
     @follows_dynamics_determinism
     @torch.no_grad()
     def inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings=1, jump_length=1, return_frames=1,
-                timesteps=None):
-        """en_diffusion.py:677-837: sample the free nodes while the fixed ones follow q(z_s | x)."""
+                timesteps=None, seeds=None):
+        """en_diffusion.py:677-837: sample the free nodes while the fixed ones follow q(z_s | x).  ``seeds``: as sample."""
+        from . import seeded
+        seeds = seeded.as_seeds(seeds, len(ligand['size']), ligand['x'].device)
+        with self._seeded(seeds, ligand['mask'], pocket['mask']):
+            return self._inpaint(ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps)
+
+    def _inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps):
+        from . import seeded
         timesteps = self.T if timesteps is None else timesteps
+        if self._rng is not None:          # u counts the jump-back blocks of the RePaint schedule
+            seeded.check_schedule(timesteps, len(self.get_repaint_schedule(resamplings, jump_length, timesteps)))
         assert 0 < return_frames <= timesteps
         assert timesteps % return_frames == 0
         assert jump_length == 1 or return_frames == 1, "Chain visualization is only implemented for jump_length=1"
@@ -627,6 +729,7 @@ class EnVariationalDiffusion(nn.Module):
         xh0_lig[:, :nd] = xh0_lig[:, :nd] - mean_known[lmask]
         xh0_pocket[:, :nd] = xh0_pocket[:, :nd] - mean_known[pmask]
 
+        self._draw_at(seeded.STAGE_PRIOR)
         z_lig, z_pocket = self.sample_combined_position_feature_noise(lmask, pmask)
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + z_pocket.size(), device=z_pocket.device)
@@ -645,7 +748,7 @@ class EnVariationalDiffusion(nn.Module):
             try:
                 g_it = self._joint_graph(st, 'inpaint', z_lig, z_pocket, s)
                 g_jump = self._joint_graph(st, 'inpaint_jump', z_lig, z_pocket, s) if len(schedule) > 1 else None
-                st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(s)
+                self._joint_start(st, z_lig, z_pocket, s)
                 for i, n_denoise in enumerate(schedule):
                     for j in range(n_denoise):
                         jump = j == n_denoise - 1 and i < len(schedule) - 1
@@ -658,12 +761,15 @@ class EnVariationalDiffusion(nn.Module):
                             out_lig[idx], out_pocket[idx] = self.unnormalize_z(st['zl'], st['zp'])
                         if jump:
                             if frame:
+                                self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
                                 s_arr = torch.full((n_samples, 1), fill_value=s, device=z_lig.device) / timesteps
                                 t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
                                 zl, zp = self.sample_p_zt_given_zs(
                                     st['zl'], st['zp'], lmask, pmask, self.inflate_batch_array(self.gamma(t_back), ligand['x']),
                                     self.inflate_batch_array(self.gamma(s_arr), ligand['x']))
                                 st['zl'].copy_(zl); st['zp'].copy_(zp); st['step'].add_(jump_length)
+                                if st['seeded']:
+                                    st['u'].add_(1)
                             s = s + jump_length
                         s -= 1
             finally:
@@ -679,7 +785,9 @@ class EnVariationalDiffusion(nn.Module):
                     s_array = s_array / timesteps
                     gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
                     # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
+                    self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_KNOWN)
                     zk_lig, zk_pocket, _, _ = self.noised_representation(xh0_lig, xh0_pocket, lmask, pmask, gamma_s)
+                    self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_REVERSE)
                     zu_lig, zu_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, z_pocket, lmask, pmask)
                     # align the COM of the noised known part with the denoised one (en_diffusion.py:751-772)
                     shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
@@ -699,19 +807,16 @@ class EnVariationalDiffusion(nn.Module):
                         t_back = torch.full((n_samples, 1), fill_value=t, device=z_lig.device) / timesteps
                         gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
                         gamma_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
+                        self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
                         z_lig, z_pocket = self.sample_p_zt_given_zs(z_lig, z_pocket, lmask, pmask, gamma_t, gamma_s)
                         s = t
                     s -= 1
 
+        self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, z_pocket, lmask, pmask, n_samples)
         self.assert_mean_zero_with_mask(torch.cat((x_lig, x_pocket), dim=0), combined_mask)
         if return_frames == 1:
-            xc = torch.cat((x_lig, x_pocket))
-            max_cog = scatter_add(xc, combined_mask, dim=0).abs().max().item()
-            if max_cog > 5e-2:
-                print(f'Warning CoG drift with error {max_cog:.3f}. Projecting the positions down.')
-                xc = self.remove_mean_batch(xc, combined_mask)
-                x_lig, x_pocket = xc[:len(x_lig)], xc[len(x_lig):]
+            x_lig, x_pocket = self._project_joint_cog_drift(x_lig, x_pocket, lmask, pmask)
         out_lig[0] = torch.cat([x_lig, h_lig], dim=1)
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lmask, pmask

@@ -22,6 +22,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+from . import seeded
 from .conditional_model import ConditionalDDPM, SimpleConditionalDDPM
 from .dynamics import EGNNDynamics
 from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_mean, num_nodes_to_batch_mask
@@ -171,13 +172,17 @@ class LigandPocketDDPM(_Base):
     @follows_dynamics_determinism
     @torch.no_grad()
     def generate_ligand_tensors(self, pocket, num_nodes_lig=None, timesteps=None, n_nodes_bias=0, n_nodes_min=0,
-                                **kwargs):
+                                seeds=None, **kwargs):
         """Everything ``generate_ligands`` does between pocket preparation and molecule building
         (lightning_modules.py:785-852): returns (xh_lig, xh_pocket, lig_mask, pocket_mask) in the original
-        pocket frame."""
+        pocket frame.  ``seeds``: one int64 per sample (seeded.py); the ligand size prior and every sampler draw then come
+        from the sample's own seed (the size by inverse CDF over p(n_lig | n_pocket))."""
         self.ddpm.eval()
+        seeds = seeded.as_seeds(seeds, len(pocket['size']), pocket['x'].device)
         pocket_com_before = scatter_mean(pocket['x'], pocket['mask'], dim=0)
-        if num_nodes_lig is None:
+        if num_nodes_lig is None and seeds is not None:
+            num_nodes_lig = seeded.size_prior(self.ddpm.size_distribution.prob, pocket['size'], seeds)
+        elif num_nodes_lig is None:
             num_nodes_lig = self.ddpm.size_distribution.sample_conditional(n1=None, n2=pocket['size'])
         num_nodes_lig = torch.clamp(num_nodes_lig + n_nodes_bias, min=n_nodes_min)
         if type(self.ddpm) == EnVariationalDiffusion:
@@ -189,10 +194,10 @@ class LigandPocketDDPM(_Base):
             lig_fixed = torch.zeros(len(lig_mask), device=self.device)
             pocket_fixed = torch.ones(len(pocket['mask']), device=self.device)
             xh_lig, xh_pocket, lig_mask, pocket_mask = self.ddpm.inpaint(
-                ligand, pocket, lig_fixed, pocket_fixed, timesteps=timesteps, **kwargs)
+                ligand, pocket, lig_fixed, pocket_fixed, timesteps=timesteps, seeds=seeds, **kwargs)
         elif type(self.ddpm) == ConditionalDDPM:
             xh_lig, xh_pocket, lig_mask, pocket_mask = self.ddpm.sample_given_pocket(
-                pocket, num_nodes_lig, timesteps=timesteps)
+                pocket, num_nodes_lig, timesteps=timesteps, seeds=seeds)
         else:
             raise NotImplementedError
         pocket_com_after = scatter_mean(xh_pocket[:, :self.x_dims], pocket_mask, dim=0)

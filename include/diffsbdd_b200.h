@@ -182,11 +182,10 @@ int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode);
  * receiver's sum is then a function of that receiver's own edges, so dsb_dynamics_forward gives bit-identical outputs
  * for bit-identical inputs (the whole batch: every graph, in the same order), weights and math mode on the same GPU
  * model with the same library build, independent of the run or process, eager launch vs. CUDA-graph replay,
- * programmatic dependent launch, workspace / output addresses and the persistent grid size.  A graph's outputs do not
- * depend bitwise on the other graphs of the batch only in math mode 0 (fp32 FFMA kernels); with any tensor-core kernel
- * (math mode != 0) the same graph denoised alone and inside another batch can differ in the last bits (measured up to
- * ~2e-6: the tensor-core edge kernels' SiLU shares one reciprocal between tile rows r and r + 8, so an edge's rounding
- * depends on the edge 8 rows away), so regenerating one graph bit for bit needs the same batch layout as well.  Results are not bit-identical
+ * programmatic dependent launch, workspace / output addresses and the persistent grid size.  A graph's outputs also do
+ * not depend bitwise on the other graphs of the batch, in any math mode: the same graph denoised alone or inside any
+ * batch, at any position, gives the same bits (the tensor-core edge kernels' shared-reciprocal SiLU groups values of one
+ * edge only in this mode), so one graph can be regenerated on its own.  Results are not bit-identical
  * across math modes, nor with the default mode.  If the edges of a call exceed edge_capacity (status[2]) the outputs are
  * invalid as in the default mode; the deterministic kernels then stop at the end of the partial buffer.  Cost: dsb_dynamics_workspace_bytes grows by a partial buffer of
  * ceil((edge_capacity + 3 (n_atoms + n_residues)) / 128) * 32 * hidden_nf floats, and dsb_dynamics_forward enqueues one
@@ -292,6 +291,31 @@ int dsb_ddpm_vlb_terms(const float* xh0_lig, const float* z_t_lig, const float* 
                        const float* net_0_pocket, const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues,
                        int64_t n_atoms, int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf,
                        float norm_value_h, float norm_bias_h, int32_t vnode_idx, float* terms, float* xh_lig_hat, void* stream);
+
+/* ---- seeded per-graph random numbers (the samplers' `seeds=` argument).  Fills out [rows, cols] (row-major fp32) so that a
+ * value depends only on (seed of its graph, draw id, role, row index within its graph, column), never on the other graphs
+ * of the batch or on the row's position in it.  This mapping is a reproducibility contract: a sampled ligand is a function
+ * of its seed, so changing any step below changes every seeded result.
+ *   role  DSB_RNG_LIGAND:  rows = n_atoms, graph g = mask_atoms[r], index i = r - (first row of g)
+ *         DSB_RNG_POCKET:  rows = n_residues over mask_residues, likewise
+ *         DSB_RNG_JOINT_X: rows = n_atoms + n_residues (ligand rows first, as the joint model's shared coordinate noise);
+ *                          a pocket row's index is (ligand rows of g) + its index among g's pocket rows
+ *         DSB_RNG_GRAPH:   rows = n_graphs, g = r, i = 0 (one row per graph, e.g. the size prior)
+ *   key      (k0, k1) = (low, high) 32-bit words of seeds[g] (int64, device)
+ *   counter  (c0, c1, c2, c3) = (column group j = col / 4, i, role | (draw >> 32) << 4, draw & 0xffffffff), draw = *draw_id
+ *            (int64, device: read at run time, so one captured graph serves every step)
+ *   words    (w0, w1, w2, w3) = Philox4x32-10(counter, key) (Random123 constants; the key is bumped after every round)
+ *   kind DSB_RNG_NORMAL:  U(w) = fmaf((float)w, 2^-32, 2^-33) in (0, 1] ((float)w rounds to nearest);
+ *                         columns 4j, 4j+1 = r0 cos(2 pi v0), r0 sin(2 pi v0) with r0 = sqrtf(-2 logf(U(w0))),
+ *                         v0 = (float)w1 * 2^-32 (sincospif(2 v0)); columns 4j+2, 4j+3 the same from (w2, w3)
+ *        DSB_RNG_UNIFORM: columns 4j+k = U(wk) in (0, 1]
+ *        DSB_RNG_BITS:    columns 4j+k = the raw word wk (bit pattern stored in the fp32 slot)
+ * Columns past `cols` of the last group are dropped.  Capturable; touches no other generator state. */
+enum { DSB_RNG_LIGAND = 0, DSB_RNG_POCKET = 1, DSB_RNG_JOINT_X = 2, DSB_RNG_GRAPH = 3 };
+enum { DSB_RNG_NORMAL = 0, DSB_RNG_UNIFORM = 1, DSB_RNG_BITS = 2 };
+int dsb_seeded_normal(float* out, int64_t cols, int32_t role, int32_t kind, const int64_t* seeds, const int64_t* draw_id,
+                      const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues,
+                      int64_t n_graphs, void* stream);
 
 const char* dsb_last_error(void);
 const char* dsb_version(void);
