@@ -6,8 +6,10 @@ import ctypes as C
 import pytest
 import torch
 
+import repaint_cases as rc
 from ddpm_cases import DDPM_CFG, DDPM_SHAPES, HIST, assert_fp64_bound, ddpm_shape, make_pocket, make_ligand
 from oracle.cpu_denoiser import OracleDynamics
+from trajectory_cases import joint_update_ref
 from diffsbdd_b200 import _native, synthetic as syn
 from diffsbdd_b200.conditional_model import ConditionalDDPM
 from diffsbdd_b200.dynamics import EGNNDynamics
@@ -212,30 +214,7 @@ def _check_fused_inpaint(shape):
     lib = _native.load()
 
     def ref(dtype, renoise):
-        """The torch ops in eager order."""
-        z_unknown_, pocket_, known_, com0_, fixed_, n1_, n2_, coef_ = (
-            x.to(dtype) for x in (z_unknown, pocket, known, com0, fixed, n1, n2, coef))
-        com_pocket = scatter_mean(pocket_[:, :3], pm)
-        xk = known_.clone()
-        xk[:, :3] = known_[:, :3] + (com_pocket - com0_)[lm]
-        zk = coef_[lm, 0:1] * xk + coef_[lm, 1:2] * n1_
-        pk = pocket_.clone()
-        mean = scatter_mean(zk[:, :3], lm)
-        zk[:, :3] = zk[:, :3] - mean[lm]
-        pk[:, :3] = pk[:, :3] - mean[pm]
-        rows = fixed_.bool()
-        cn = scatter_mean(zk[rows][:, :3], lm[rows], dim_size=B)
-        cd = scatter_mean(z_unknown_[rows][:, :3], lm[rows], dim_size=B)
-        dx = cd - cn
-        zk[:, :3] = zk[:, :3] + dx[lm]
-        pk[:, :3] = pk[:, :3] + dx[pm]
-        want = zk * fixed_[:, None] + z_unknown_ * (1 - fixed_[:, None])
-        if renoise:
-            want = coef_[lm, 2:3] * want + coef_[lm, 3:4] * n2_
-            m2 = scatter_mean(want[:, :3], lm)
-            want[:, :3] = want[:, :3] - m2[lm]
-            pk[:, :3] = pk[:, :3] - m2[pm]
-        return want, pk
+        return rc.inpaint_update_ref(z_unknown, pocket, known, com0, fixed, n1, n2 if renoise else None, coef, lm, pm, dtype)
 
     for renoise in (False, True):
         want, pk = ref(torch.float32, renoise)
@@ -395,12 +374,6 @@ def test_joint_repaint_inpaint_denoiser_calls_match_oracle():
     assert com.abs().max() < 5e-2 * max(1.0, float(out[1][:, :3].abs().max()))
 
 
-def _joint_ref_noise(nx, lm, pm):
-    """COM-free position noise as sample_center_gravity_zero_gaussian_batch builds it (en_diffusion.py:940-944)."""
-    cm = torch.cat((lm, pm))
-    return nx - scatter_mean(nx, cm)[cm]
-
-
 def test_fused_joint_kernels_match_torch_ops():
     """dsb_ddpm_joint_update / dsb_ddpm_joint_inpaint_update against the torch ops of the eager joint sampler
     (en_diffusion.py:503-557, :741-807), ragged graphs, partially fixed pocket, with and without the jump back, at every
@@ -415,7 +388,6 @@ def _check_fused_joint(shape):
     A, R, B = 10, 10, len(n_lig)
     lm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_lig)).cuda()
     pm = torch.repeat_interleave(torch.arange(B), torch.tensor(n_poc)).cuda()
-    cm = torch.cat((lm, pm))
     NL, NP = sum(n_lig), sum(n_poc)
     rnd = lambda *shape: torch.randn(shape, generator=g).cuda()
     zl, zp, el, ep = rnd(NL, 3 + A), rnd(NP, 3 + R), rnd(NL, 3 + A), rnd(NP, 3 + R)
@@ -426,14 +398,7 @@ def _check_fused_joint(shape):
     P = lambda t: t.data_ptr()
 
     def ref_update(dtype):
-        zl_, zp_, el_, ep_, nx_, nhl_, nhp_, coef3_ = (x.to(dtype) for x in (zl, zp, el, ep, nx, nhl, nhp, coef3))
-        ex = _joint_ref_noise(nx_, lm, pm)
-        eps_l, eps_p = torch.cat((ex[:NL], nhl_), 1), torch.cat((ex[NL:], nhp_), 1)
-        wl = zl_ / coef3_[lm, 0:1] - coef3_[lm, 1:2] * el_ + coef3_[lm, 2:3] * eps_l
-        wp = zp_ / coef3_[pm, 0:1] - coef3_[pm, 1:2] * ep_ + coef3_[pm, 2:3] * eps_p
-        mean = scatter_mean(torch.cat((wl[:, :3], wp[:, :3])), cm)
-        wl[:, :3] -= mean[lm]; wp[:, :3] -= mean[pm]
-        return wl, wp
+        return joint_update_ref(zl, zp, el, ep, (nx, nhl, nhp), coef3, lm, pm, dtype)
 
     wl, wp = ref_update(torch.float32)
     wl64, wp64 = ref_update(torch.float64)
@@ -452,28 +417,7 @@ def _check_fused_joint(shape):
     n3 = (rnd(NL + NP, 3), rnd(NL, A), rnd(NP, R))
 
     def ref_inpaint(dtype, jump):
-        zl_, zp_, nx_, nhl_, nhp_, x0l_, x0p_, fl_, fp_, coef4_ = (
-            x.to(dtype) for x in (zl, zp, nx, nhl, nhp, x0l, x0p, fl, fp, coef4))
-        ex = _joint_ref_noise(nx_, lm, pm)
-        eps_l, eps_p = torch.cat((ex[:NL], nhl_), 1), torch.cat((ex[NL:], nhp_), 1)
-        zkl = coef4_[lm, 0:1] * x0l_ + coef4_[lm, 1:2] * eps_l
-        zkp = coef4_[pm, 0:1] * x0p_ + coef4_[pm, 1:2] * eps_p
-        sel_l, sel_p = fl_.bool(), fp_.bool()
-        idx = torch.cat((lm[sel_l], pm[sel_p]))
-        com_u = scatter_mean(torch.cat((zl_[sel_l][:, :3], zp_[sel_p][:, :3])), idx, dim_size=B)
-        com_k = scatter_mean(torch.cat((zkl[sel_l][:, :3], zkp[sel_p][:, :3])), idx, dim_size=B)
-        shift = com_u - com_k
-        zkl[:, :3] += shift[lm]; zkp[:, :3] += shift[pm]
-        wl = zkl * fl_[:, None] + zl_ * (1 - fl_[:, None])
-        wp = zkp * fp_[:, None] + zp_ * (1 - fp_[:, None])
-        if jump:
-            n3x, n3l, n3p = (x.to(dtype) for x in n3)
-            e3 = _joint_ref_noise(n3x, lm, pm)
-            wl = coef4_[lm, 2:3] * wl + coef4_[lm, 3:4] * torch.cat((e3[:NL], n3l), 1)
-            wp = coef4_[pm, 2:3] * wp + coef4_[pm, 3:4] * torch.cat((e3[NL:], n3p), 1)
-            mean = scatter_mean(torch.cat((wl[:, :3], wp[:, :3])), cm)
-            wl[:, :3] -= mean[lm]; wp[:, :3] -= mean[pm]
-        return wl, wp
+        return rc.joint_inpaint_update_ref(zl, zp, x0l, x0p, fl, fp, (nx, nhl, nhp), n3 if jump else None, coef4, lm, pm, dtype)
 
     for jump in (False, True):
         wl, wp = ref_inpaint(torch.float32, jump)

@@ -60,6 +60,7 @@ import pytest
 import torch
 
 from ddpm_cases import assert_fp64_bound
+from repaint_cases import joint_step_coefficients
 from helpers import ATOL, RTOL, assert_close
 from stress_cases import column_errors
 from trajectory_cases import (COND_SEED, JOINT_LIG, JOINT_POC, JOINT_SEED, PLANT_CFG, T, candidate_pairs, compare_edges,
@@ -126,15 +127,6 @@ def test_recorder_runs_the_production_sampler(traj):
     assert torch.isfinite(rec['z'][T]).all() and torch.isfinite(rec['pocket'][T]).all()
 
 
-def _joint_step_coefficients(ddpm, s, t, target):
-    """The coefficient ops of the eager EnVariationalDiffusion.sample_p_zs_given_zt."""
-    gamma_s, gamma_t = ddpm.gamma(s), ddpm.gamma(t)
-    sigma2_ts, sigma_ts, alpha_ts = ddpm.sigma_and_alpha_t_given_s(gamma_t, gamma_s, target)
-    sigma_s = ddpm.sigma(gamma_s, target_tensor=target)
-    sigma_t = ddpm.sigma(gamma_t, target_tensor=target)
-    return torch.cat([alpha_ts, sigma2_ts / alpha_ts / sigma_t, sigma_ts * sigma_s / sigma_t], 1)
-
-
 def test_step_tables_every_step(traj):
     ddpm, rec, n = traj.ddpm, traj.rec, traj.n
     if traj.joint:
@@ -154,7 +146,7 @@ def test_step_tables_every_step(traj):
         assert abs(float(rec['t'][k][0]) - (s + 1) / T) <= 2 * ulp32((s + 1) / T)
         assert torch.equal(torch.round(rec['t'][k] * T).long(), torch.full_like(s_array, s + 1, dtype=torch.long))
         if traj.joint:
-            want = _joint_step_coefficients(ddpm, s_array, t_array, target)
+            want = joint_step_coefficients(ddpm, s_array, t_array, target)
         else:
             want = torch.cat(ddpm._step_coefficients(ddpm.gamma(s_array), ddpm.gamma(t_array), target), 1)
         assert torch.equal(rec['coef3'][k], want), \
