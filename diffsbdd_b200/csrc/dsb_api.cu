@@ -969,10 +969,10 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
   };
 #define DSB_TRY(expr) do { if (int e_ = (expr)) return e_; } while (0)
   const int mm = (tc_width_supported(H) && !c.sin_embedding) ? dyn->math_mode : 0;      // sin_embedding: fp32 FFMA kernels only
-  const bool f16 = (mm & 8) != 0;
+  const TcFormat fmt = !(mm & 8) ? TcFormat::TF32x3 : (mm & 16) ? TcFormat::F16x1 : TcFormat::F16x3;
   const bool det = dyn->deterministic != 0;
   auto gemm = [&](const GemmArgs& ga, const TcImage& img, int n_tile_off = 0) -> int {
-    return ((mm & 1) && img.t_hi) ? launch_tc_node_gemm(dyn, ga, img, n_tile_off, f16, status, s) : launch_node_gemm(ga, s);
+    return ((mm & 1) && img.t_hi) ? launch_tc_node_gemm(dyn, ga, img, n_tile_off, fmt, status, s) : launch_node_gemm(ga, s);
   };
 
   // test hook (dsb_dynamics_set_stop_after): `ops` counts the operations enqueued so far; DSB_OP() before each one returns
@@ -1014,7 +1014,7 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
       }
       mark(KC_EDGE_GCL);
       DSB_OP();
-      DSB_TRY((mm & 2) ? launch_tc_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, f16, status, s) : launch_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, s));
+      DSB_TRY((mm & 2) ? launch_tc_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, fmt, status, s) : launch_edge_gcl(dyn, dm, ws, G, xcur, pv_gcl, s));
       if (det) {              // fixed-order receiver sums: agg = per-receiver sums of the chunk partials (one slot per chunk)
         DSB_OP(); DSB_TRY(launch_segment_reduce(ws, dm.N, H / 4, 1, reinterpret_cast<float4*>(ws.agg), s));
         launches += 1;
@@ -1037,7 +1037,7 @@ int dsb_dynamics_forward(dsb_dynamics* dyn, const float* xh_atoms, const float* 
     DSB_OP(); DSB_TRY(gemm(g4, Q.iW1));
     mark(KC_EDGE_COORD);
     DSB_OP();
-    DSB_TRY((mm & 4) ? launch_tc_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, f16, status, s) : launch_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, s));
+    DSB_TRY((mm & 4) ? launch_tc_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, fmt, status, s) : launch_edge_coord(dyn, dm, ws, Q, xcur, pv_coord, s));
     if (det && dm.n_coord_rows > 0) {   // xagg rows of the moving nodes; the tensor-core kernel keeps one slot per chunk and MLP
       DSB_OP(); DSB_TRY(launch_segment_reduce(ws, dm.n_coord_rows, 1, (mm & 4) ? nm : 1, ws.xagg, s));
       launches += 1;
@@ -1072,7 +1072,8 @@ int dsb_set_programmatic_launch(int enable) {
 
 int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode) {
   if (!dyn) { set_error("null handle"); return DSB_ERR_INVALID_ARGUMENT; }
-  if (mode < 0 || mode > 15) { set_error("math mode must be a bitmask in [0,15]"); return DSB_ERR_INVALID_ARGUMENT; }
+  if (mode < 0 || mode > 31) { set_error("math mode must be a bitmask in [0,31]"); return DSB_ERR_INVALID_ARGUMENT; }
+  if ((mode & 16) && !(mode & 8)) { set_error("math mode bit 16 (single fp16 product) needs bit 8 (fp16 operands)"); return DSB_ERR_INVALID_ARGUMENT; }
   if (mode != 0 && dyn->cfg.sin_embedding) { set_error("sin_embedding is built in the fp32 FFMA kernels only (math mode 0)"); return DSB_ERR_UNSUPPORTED_CONFIG; }
   if (mode != 0 && !tc_width_supported(dyn->cfg.hidden_nf)) { set_error("the tensor-core kernels are built for hidden_nf 128, 192 and 256 only"); return DSB_ERR_UNSUPPORTED_CONFIG; }
   dyn->math_mode = mode;

@@ -117,7 +117,8 @@ struct dsb_dynamics {
   float* blob = nullptr;
   size_t blob_floats = 0;
   int num_sms = 132;
-  int math_mode = 0;         // bitmask: 1 node GEMMs, 2 edge_gcl, 4 edge_coord on wgmma (H in {128,192,256}); 8: 3xFP16 split instead of 3xTF32
+  int math_mode = 0;         // bitmask: 1 node GEMMs, 2 edge_gcl, 4 edge_coord on wgmma (H in {128,192,256}); 8: 3xFP16 split instead of 3xTF32;
+                             //   16 (with 8): single fp16 product x_hi.w_hi instead of the 3xFP16 split
   int deterministic = 0;     // 1: fixed-order receiver sums (chunk partials + segment reduce) instead of atomics
   int last_launches = 0;     // kernels only
   int last_memsets = 0;
@@ -210,16 +211,19 @@ int configure_edge_kernels(int H);
 int launch_segment_reduce(const Workspace& ws, int n_rows, int ld4, int spc, float4* out, cudaStream_t s);
 
 // ---- tensor-core path (dsb_tc.cu) --------------------------------------------------------------------
+// operand format of the wgmma contractions (math-mode bits 8 and 16): 3-product split in tf32 or fp16, or the single fp16
+// product x_hi.w_hi
+enum class TcFormat { TF32x3, F16x3, F16x1 };
 void launch_pack_b_image(float* hi, float* lo, const float* src, int lds, int scol, int n_rows, int n_dst_off, int K, int tn);
 void launch_pack_b_image_f16(float* hi, float* lo, const float* src, int lds, int scol, int n_rows, int n_dst_off, int K, float scale, int tn);
 void launch_absmax(const float* src, int lds, int scol, int n_rows, int K, unsigned* out);
 int configure_tc_kernels(int H);
 bool tc_width_supported(int H);     // hidden_nf values with tensor-core kernels (128, 192, 256)
-int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage& w, int n_tile_off, bool f16, int32_t* status,
+int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage& w, int n_tile_off, TcFormat fmt, int32_t* status,
                         cudaStream_t s);
-int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const float4* x, PView pv, bool f16,
+int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const float4* x, PView pv, TcFormat fmt,
                        int32_t* status, cudaStream_t s);
-int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w, const float4* x, PView pv, bool f16,
+int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w, const float4* x, PView pv, TcFormat fmt,
                          int32_t* status, cudaStream_t s);
 
 // ---- device math helpers ----------------------------------------------------------------------------

@@ -1,5 +1,5 @@
-// Tensor-core (wgmma, sm_90a) kernels of the denoiser: 3-product split contractions (3xFP16 or 3xTF32 operands) with fp32
-// accumulation in registers.
+// Tensor-core (wgmma, sm_90a) kernels of the denoiser: 3-product split contractions (3xFP16 or 3xTF32 operands), or the
+// single fp16 product (1xFP16), with fp32 accumulation in registers.
 //
 //   tc_node_gemm_kernel    — C = act([A1 | A2/div] @ W + bias) (+R)   (node MLPs, merged first layers)
 //   tc_edge_kernel<0,..>   — GCL.edge_model + receiver sums           (egnn_new.py:31-52)
@@ -93,7 +93,7 @@ struct TcGemmArgs {
   float* C; int ldc; int M; int Nn; int act;
   float* Z; int ldz;
   int dead_mt; int dead_nt;                    // tiles with m-tile >= dead_mt and n-tile < dead_nt are skipped (dead_nt == 0: none)
-  float inv_scale;                             // 3xFP16: 1 / (X_SCALE * weight scale); 1 for 3xTF32
+  float inv_scale;                             // 3xFP16 / 1xFP16: 1 / (X_SCALE * weight scale); 1 for 3xTF32
 };
 
 // live-tile enumeration: region A = m-tiles [0, dead_mt) x all n-tiles, region B = m-tiles [dead_mt, ntm) x n-tiles [dead_nt, ntn)
@@ -111,9 +111,10 @@ struct TileMap {
   }
 };
 
-template <bool F16, int H>
+template <TcFormat FMT, int H>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs g) {
   using G = Geo<H>;
+  constexpr bool F16 = FMT != TcFormat::TF32x3;
   constexpr int TN = H, HPC = F16 ? 2 : 1;     // 32-k halves per pipeline chunk
   extern __shared__ uint8_t smem_raw[];
   char* const stages = align1024(smem_raw);
@@ -129,7 +130,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
   if (threadIdx.x == 0) control_init(ctl);
   __syncthreads();
   pdl_wait();
-  const WeightStream<H> wst{ctl, stages};
+  const WeightStream<FMT, H> wst{ctl, stages};
   auto issue_w = [&](uint32_t q) {             // weight chunk of global chunk index q
     const int it = (int)(q / chunks), kc = (int)(q - (uint32_t)it * chunks);
     int mt, nt;
@@ -180,14 +181,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_node_gemm_kernel(TcGemmArgs 
             const float dv = g.deg2 ? (float)max(m < g.M ? g.deg2[m] : 1, 1) : g.div2;
             x.x = __fdiv_rn(x.x, dv); x.y = __fdiv_rn(x.y, dv); x.z = __fdiv_rn(x.z, dv); x.w = __fdiv_rn(x.w, dv);
           }
-          store_pair<F16>(st + piece_offset<F16>(r0 + i, hf, pc), pk2(x.x, x.y), pk2(x.z, x.w));
+          store_pair<FMT>(st + piece_offset<F16>(r0 + i, hf, pc), pk2(x.x, x.y), pk2(x.z, x.w));
         }
       }
       fence_proxy_async();                     // generic-proxy operand stores -> visible to the wgmma (async proxy)
       wg_sync(wg);
       mbar_wait(&ctl->full_w[s], (q >> 1) & 1);
       wgmma_fence();
-      mma_chunk<F16, H>(acc, st, wg, kc == 0);
+      mma_chunk<FMT, H>(acc, st, wg, kc == 0);
       wgmma_commit();
       trk.release_prev(ctl, (int)q, lane == 0);
     }
@@ -267,7 +268,7 @@ struct TcEdgeArgs {
   float norm_constant, coords_range; int use_tanh;
   float* agg;                                // GCL: [N][H] raw sums
   float4* xagg;                              // coord: [N] raw sums of trans
-  float inv_scale[2];                        // 3xFP16: 1 / (X_SCALE * W2 scale) per MLP; 1 for 3xTF32
+  float inv_scale[2];                        // 3xFP16 / 1xFP16: 1 / (X_SCALE * W2 scale) per MLP; 1 for 3xTF32
   float* part;                               // deterministic variant: chunk partials (Workspace::part) instead of agg / xagg
   int vcap;                                  // deterministic variant: virtual rows covered by vmap / part (Workspace::vcap)
 };
@@ -335,9 +336,10 @@ struct ScalarSteps {
 // DET (deterministic mode): the same chunk sums are stored, not added, into slot (virtual chunk) of a.part (coord: slot
 // chunk * nm + m, one float4); launch_segment_reduce then sums each receiver's slots in ascending order.  The chunk sums
 // have a fixed content and order, so the receiver sums depend on the receiver's own edges only.
-template <bool COORD, bool F16, int H, bool TB, bool DET = false>
+template <bool COORD, TcFormat FMT, int H, bool TB, bool DET = false>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
   using G = Geo<H>;
+  constexpr bool F16 = FMT != TcFormat::TF32x3;
   constexpr int HPC = F16 ? 2 : 1;             // 32-k halves per pipeline chunk
   constexpr int chunks = H / (TKC * HPC);
   extern __shared__ uint8_t smem_raw[];
@@ -365,7 +367,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
   if (n_my == 0) return;
   auto unit_tile = [&](int j, int& m) { const int v = blockIdx.x + j * gridDim.x, t = v / nm; m = v - t * nm; return t; };
   const uint32_t total = (uint32_t)(n_my * chunks);
-  const WeightStream<H> wst{ctl, stages};
+  const WeightStream<FMT, H> wst{ctl, stages};
   auto issue_w = [&](uint32_t q) {
     const int j = (int)(q / chunks), kc = (int)(q - (uint32_t)j * chunks);
     int m;
@@ -424,7 +426,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
           u01 = add2(u01, pk2(t4.x, t4.y)); u23 = add2(u23, pk2(t4.z, t4.w));
         }
         silu_pair<(DSB_SILU_PAIR & 1) != 0, (DSB_SILU_QUAD & 1) != 0>(u01, u23);
-        store_pair<F16>(st + piece_offset<F16>(r0 + i, hf, pc), u01, u23);
+        store_pair<FMT>(st + piece_offset<F16>(r0 + i, hf, pc), u01, u23);
       }
     }
   };
@@ -438,7 +440,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
     wg_sync(wg);
     mbar_wait(&ctl->full_w[s], (q >> 1) & 1);
     wgmma_fence();
-    mma_chunk<F16, H>(acc, stages + (size_t)s * G::STAGE_BYTES, wg, kc == 0);
+    mma_chunk<FMT, H>(acc, stages + (size_t)s * G::STAGE_BYTES, wg, kc == 0);
     wgmma_commit();
     trk.release_prev(ctl, (int)q, lane == 0);
     ++q;
@@ -460,7 +462,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_edge_kernel(TcEdgeArgs a) {
     EdgeScalars* sc_next = &ex->sc[(j + 1) & 1];
     int m_next;
     const int e0_next = unit_tile(j + 1, m_next) * TM;      // past the last unit: rows >= E, all padding
-#pragma unroll (F16 ? chunks : 1)
+    // the 1xFP16 GCL kernel at H = 256 with the type table stays rolled: fully unrolled, ptxas spills there
+#pragma unroll ((F16 && !(FMT == TcFormat::F16x1 && !COORD && TB && H == 256)) ? chunks : 1)
     for (int kc = 0; kc < chunks - 1; ++kc) {
       issue(kc);
       for (int k = kc * kSteps / (chunks - 1); k < (kc + 1) * kSteps / (chunks - 1); ++k)
@@ -607,35 +610,43 @@ static int dispatch_width(int H, Fn&& fn) {
   }
 }
 
-int configure_tc_kernels(int H) {
+// run `fn.template operator()<F, H>()` for the run-time operand format and width
+template <typename Fn>
+static int dispatch_tc(TcFormat f, int H, Fn&& fn) {
   return dispatch_width(H, [&]<int W>() -> int {
-    const int gs = (int)gemm_smem_bytes<W>(), es = (int)edge_smem_bytes<W>();
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_node_gemm_kernel<false, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, gs));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_node_gemm_kernel<true, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, gs));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, false, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, true, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, false, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, true, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
-    return 0;
+    switch (f) {
+      case TcFormat::TF32x3: return fn.template operator()<TcFormat::TF32x3, W>();
+      case TcFormat::F16x3: return fn.template operator()<TcFormat::F16x3, W>();
+      default: return fn.template operator()<TcFormat::F16x1, W>();
+    }
   });
 }
 
-int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage& w, int n_tile_off, bool f16, int32_t* status,
+int configure_tc_kernels(int H) {
+  for (const TcFormat f : {TcFormat::TF32x3, TcFormat::F16x3, TcFormat::F16x1}) {
+    const int e = dispatch_tc(f, H, [&]<TcFormat F, int W>() -> int {
+      const int gs = (int)gemm_smem_bytes<W>(), es = (int)edge_smem_bytes<W>();
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_node_gemm_kernel<F, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, gs));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, F, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, F, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, F, W, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, F, W, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, F, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<false, F, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, F, W, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      DSB_CUDA_OK(cudaFuncSetAttribute(tc_edge_kernel<true, F, W, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, es));
+      return 0;
+    });
+    if (e) return e;
+  }
+  return 0;
+}
+
+int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage& w, int n_tile_off, TcFormat fmt, int32_t* status,
                         cudaStream_t s) {
   (void)status;
   if (g.M == 0) return 0;
+  const bool f16 = fmt != TcFormat::TF32x3;
   const int K = g.K1 + g.K2, TN = d->cfg.hidden_nf;
   if ((g.Nn % TN) || (K % TKC16) || (g.K1 % TKC16) || (g.lda1 % 4) || (g.ldc % 4)) {
     set_error("tc_node_gemm: unsupported shape K1=%d K2=%d Nn=%d", g.K1, g.K2, g.Nn);
@@ -653,15 +664,16 @@ int launch_tc_node_gemm(const dsb_dynamics* d, const GemmArgs& g, const TcImage&
   const int dmt_ = a.dead_nt > 0 ? (a.dead_mt < ntm_ ? a.dead_mt : ntm_) : ntm_;
   const int n_tiles = dmt_ * ntn_ + (ntm_ - dmt_) * (ntn_ - a.dead_nt);
   const int grid = n_tiles < d->num_sms ? n_tiles : d->num_sms;
-  return dispatch_width(TN, [&]<int W>() -> int {
-    DSB_CUDA_OK(launch_k(f16 ? tc_node_gemm_kernel<true, W> : tc_node_gemm_kernel<false, W>, grid, TC_THREADS, gemm_smem_bytes<W>(), s, a));
+  return dispatch_tc(fmt, TN, [&]<TcFormat F, int W>() -> int {
+    DSB_CUDA_OK(launch_k(tc_node_gemm_kernel<F, W>, grid, TC_THREADS, gemm_smem_bytes<W>(), s, a));
     return 0;
   });
 }
 
-int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const float4* x, PView pv, bool f16,
+int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const GclW& w, const float4* x, PView pv, TcFormat fmt,
                        int32_t* status, cudaStream_t s) {
   (void)status;
+  const bool f16 = fmt != TcFormat::TF32x3;
   TcEdgeArgs a = {};
   a.P = pv.P; a.ldp = pv.ldp; a.x = x; a.cent = ws.cent; a.gid = ws.gid; a.vrow_ptr = ws.vrow_ptr; a.vmap = ws.vmap; a.n_rows = dm.N;
   a.erow = ws.erow; a.ecol = ws.ecol; a.ed0 = ws.ed0; a.NL = dm.NL; a.nm = 1;
@@ -670,20 +682,18 @@ int launch_tc_edge_gcl(const dsb_dynamics* d, const Dims& dm, const Workspace& w
   a.wr[0] = w.wr; a.wr0[0] = w.wr0; a.tb[0] = w.tb; a.b2[0] = w.b2;
   a.wa = w.wa; a.ba = w.ba; a.agg = ws.agg; a.part = ws.part; a.vcap = ws.vcap;
   const bool det = d->deterministic != 0;
-  return dispatch_width(d->cfg.hidden_nf, [&]<int W>() -> int {
-    auto kern = w.tb ? (f16 ? tc_edge_kernel<false, true, W, true> : tc_edge_kernel<false, false, W, true>)
-                     : (f16 ? tc_edge_kernel<false, true, W, false> : tc_edge_kernel<false, false, W, false>);
-    if (det)
-      kern = w.tb ? (f16 ? tc_edge_kernel<false, true, W, true, true> : tc_edge_kernel<false, false, W, true, true>)
-                  : (f16 ? tc_edge_kernel<false, true, W, false, true> : tc_edge_kernel<false, false, W, false, true>);
+  return dispatch_tc(fmt, d->cfg.hidden_nf, [&]<TcFormat F, int W>() -> int {
+    auto kern = w.tb ? tc_edge_kernel<false, F, W, true> : tc_edge_kernel<false, F, W, false>;
+    if (det) kern = w.tb ? tc_edge_kernel<false, F, W, true, true> : tc_edge_kernel<false, F, W, false, true>;
     DSB_CUDA_OK(launch_k(kern, d->num_sms, TC_THREADS, edge_smem_bytes<W>(), s, a));
     return 0;
   });
 }
 
-int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w, const float4* x, PView pv, bool f16,
+int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace& ws, const EquivW& w, const float4* x, PView pv, TcFormat fmt,
                          int32_t* status, cudaStream_t s) {
   (void)status;
+  const bool f16 = fmt != TcFormat::TF32x3;
   const dsb_config& c = d->cfg;
   TcEdgeArgs a = {};
   a.nm = c.reflection_equivariant ? 1 : 2;
@@ -698,12 +708,9 @@ int launch_tc_edge_coord(const dsb_dynamics* d, const Dims& dm, const Workspace&
   a.wa = w.w3; a.ba = nullptr;
   a.norm_constant = c.norm_constant; a.coords_range = c.coords_range; a.use_tanh = c.tanh; a.xagg = ws.xagg; a.part = ws.part; a.vcap = ws.vcap;
   const bool det = d->deterministic != 0;
-  return dispatch_width(c.hidden_nf, [&]<int W>() -> int {
-    auto kern = w.tb[0] ? (f16 ? tc_edge_kernel<true, true, W, true> : tc_edge_kernel<true, false, W, true>)
-                        : (f16 ? tc_edge_kernel<true, true, W, false> : tc_edge_kernel<true, false, W, false>);
-    if (det)
-      kern = w.tb[0] ? (f16 ? tc_edge_kernel<true, true, W, true, true> : tc_edge_kernel<true, false, W, true, true>)
-                     : (f16 ? tc_edge_kernel<true, true, W, false, true> : tc_edge_kernel<true, false, W, false, true>);
+  return dispatch_tc(fmt, c.hidden_nf, [&]<TcFormat F, int W>() -> int {
+    auto kern = w.tb[0] ? tc_edge_kernel<true, F, W, true> : tc_edge_kernel<true, F, W, false>;
+    if (det) kern = w.tb[0] ? tc_edge_kernel<true, F, W, true, true> : tc_edge_kernel<true, F, W, false, true>;
     DSB_CUDA_OK(launch_k(kern, d->num_sms, TC_THREADS, edge_smem_bytes<W>(), s, a));
     return 0;
   });

@@ -1,9 +1,11 @@
 // wgmma / mbarrier / bulk-copy PTX wrappers and the operand-format helpers of the tensor-core path (sm_90a).
 //
-// Numerics: every contraction is a 3-product split accumulated in fp32 registers by wgmma, in one of two operand formats:
+// Numerics: every contraction is accumulated in fp32 registers by wgmma, in one of three operand formats (TcFormat):
 //   3xTF32 (tf32 operands, 4 B/operand element, 8-bit exponent: range-robust), or
 //   3xFP16 (f16 operands,  2 B/operand element: half the shared-memory operand traffic and twice the MMA rate; operands are
-//           pre-scaled by powers of two so residuals stay in fp16's normal range; |x| > 65504 -> inf -> NaN flag of the output).
+//           pre-scaled by powers of two so residuals stay in fp16's normal range; |x| > 65504 -> inf -> NaN flag of the output),
+//   1xFP16 (the single product a_hi.b_hi of the 3xFP16 operands: a third of the wgmmas, no residual tile and no low weight
+//           image; fp16-grade accuracy, 2^-11 relative per operand; same range limit as 3xFP16).
 // 3xTF32:
 //     a = a_hi + a_lo,  a_hi = cvt.rna.tf32(a),  a_lo = a - a_hi   (exact; the MMA truncates a_lo to 11 bits: 2^-23 |a|)
 //     a.b ~= a_lo.b_hi + a_hi.b_lo + a_hi.b_hi                       (dropped a_lo.b_lo ~ 2^-24 |a||b|)
@@ -111,10 +113,10 @@ __device__ __forceinline__ void acc_fence(float (&d)[R]) {
 }
 
 // The 12 wgmmas of one K-chunk held in stage memory `st` (A_hi | A_lo | W_hi | W_lo) for the 64 rows of warpgroup wg:
-// 4 k-steps x 3 split products into d; the first product of a tile's first chunk overwrites d.  first_chunk only sets the
-// scale-d predicate of one instruction: no branch around the wgmmas (a divergent path between a wgmma and its wait makes
-// ptxas serialise the pipeline).
-template <bool F16, int H>
+// 4 k-steps x 3 split products into d (1xFP16: 4 k-steps x the A_hi.W_hi product); the first product of a tile's first
+// chunk overwrites d.  first_chunk only sets the scale-d predicate of one instruction: no branch around the wgmmas (a
+// divergent path between a wgmma and its wait makes ptxas serialise the pipeline).
+template <TcFormat FMT, int H>
 __device__ __forceinline__ void mma_chunk(float (&d)[H / 2], const char* st, int wg, bool first_chunk) {
   using G = Geo<H>;
   const uint32_t xhi = smem_u32(st) + (uint32_t)(wg * WG_ROWS * 128), xlo = xhi + A_CHUNK_BYTES;
@@ -123,7 +125,9 @@ __device__ __forceinline__ void mma_chunk(float (&d)[H / 2], const char* st, int
   for (int ks = 0; ks < 4; ++ks) {       // 4 k-steps of 32 bytes per 128-byte row (K=8 tf32 or K=16 fp16 each)
     const uint32_t ko = ks * 32;
     const uint32_t acc = (first_chunk && ks == 0) ? 0u : 1u;
-    if constexpr (F16) {
+    if constexpr (FMT == TcFormat::F16x1) {
+      Wgmma<H>::f16(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(whi + ko), acc);
+    } else if constexpr (FMT == TcFormat::F16x3) {
       Wgmma<H>::f16(d, wgmma_desc_sw128(xlo + ko), wgmma_desc_sw128(whi + ko), acc);
       Wgmma<H>::f16(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(wlo + ko), 1u);
       Wgmma<H>::f16(d, wgmma_desc_sw128(xhi + ko), wgmma_desc_sw128(whi + ko), 1u);
@@ -154,14 +158,18 @@ __device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cas
 
 // Producer-side store of 4 consecutive k-values of one tile row at `dst` (stage base + swizzled offset of the row piece):
 //   TF32: 16-byte stores (hi tile, lo tile A_CHUNK_BYTES further)
-//   FP16: 8-byte stores
+//   FP16: 8-byte stores (1xFP16: the hi tile only, no residual)
 // An FP16 activation beyond the fp16 range becomes inf here and reaches the output as NaN -> the NaN guard of the
 // denoiser raises; 3xTF32 has no such limit.
-template <bool F16>
+template <TcFormat FMT>
 __device__ __forceinline__ void store_pair(char* dst, f32x2 u01, f32x2 u23) {
   float x0, x1, x2, x3;
   upk2(u01, x0, x1); upk2(u23, x2, x3);
-  if constexpr (F16) {
+  if constexpr (FMT == TcFormat::F16x1) {
+    uint2 hv;
+    hv.x = h2_bits(__floats2half2_rn(x0, x1)); hv.y = h2_bits(__floats2half2_rn(x2, x3));
+    *reinterpret_cast<uint2*>(dst) = hv;
+  } else if constexpr (FMT == TcFormat::F16x3) {
     const __half2 h0 = __floats2half2_rn(x0, x1), h1 = __floats2half2_rn(x2, x3);
     float l0, l1, l2, l3;
     residual_f16(h2_bits(h0), x0, x1, l0, l1); residual_f16(h2_bits(h1), x2, x3, l2, l3);
@@ -184,7 +192,8 @@ __device__ __forceinline__ uint32_t piece_offset(int r, int hf, int p) {
 }
 
 // ---- weight pipeline --------------------------------------------------------------------------------------------------
-// Stage s holds one K-chunk: A_hi | A_lo (built by the warpgroups, each its own 64 rows) | W_hi | W_lo (bulk copies).
+// Stage s holds one K-chunk: A_hi | A_lo (built by the warpgroups, each its own 64 rows) | W_hi | W_lo (bulk copies);
+// 1xFP16 leaves A_lo and W_lo unused.
 // full_w[s]: the weight chunk has landed (1 arrive + tx bytes).  empty[s]: the wgmmas that read the stage have completed
 // in all 8 warps of both warpgroups (one arrive per warp), so the next weight chunk may be copied in.
 struct Control {
@@ -199,7 +208,7 @@ __device__ __forceinline__ void control_init(Control* c) {
 
 // Sequence of K-chunks g = 0, 1, ... of a CTA (all tiles in order), issued by lane 0 of the weight warp: chunk g goes into
 // stage g % 2 once chunk g - 2 (same stage) has been consumed by both warpgroups.
-template <int H>
+template <TcFormat FMT, int H>
 struct WeightStream {
   Control* ctl;
   char* stages;
@@ -208,9 +217,14 @@ struct WeightStream {
     const int s = g & 1;
     if (g >= NSTAGE) mbar_wait(&ctl->empty[s], ((g >> 1) - 1) & 1);
     char* st = stages + (size_t)s * G::STAGE_BYTES + 2 * A_CHUNK_BYTES;
-    mbar_arrive_expect_tx(&ctl->full_w[s], 2 * G::B_CHUNK_BYTES);
-    bulk_g2s(st, hi, G::B_CHUNK_BYTES, &ctl->full_w[s]);
-    bulk_g2s(st + G::B_CHUNK_BYTES, lo, G::B_CHUNK_BYTES, &ctl->full_w[s]);
+    if constexpr (FMT == TcFormat::F16x1) {       // W_hi only
+      mbar_arrive_expect_tx(&ctl->full_w[s], G::B_CHUNK_BYTES);
+      bulk_g2s(st, hi, G::B_CHUNK_BYTES, &ctl->full_w[s]);
+    } else {
+      mbar_arrive_expect_tx(&ctl->full_w[s], 2 * G::B_CHUNK_BYTES);
+      bulk_g2s(st, hi, G::B_CHUNK_BYTES, &ctl->full_w[s]);
+      bulk_g2s(st + G::B_CHUNK_BYTES, lo, G::B_CHUNK_BYTES, &ctl->full_w[s]);
+    }
   }
 };
 

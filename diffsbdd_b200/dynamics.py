@@ -164,7 +164,8 @@ class EGNNDynamics(nn.Module):
         self._status: Optional[torch.Tensor] = None
         self.defer_status_check = False    # samplers that CUDA-graph the loop check once at the end
         # arithmetic path: bitmask 1 node GEMMs | 2 edge kernel | 4 coordinate kernel on wgmma, 8 = 3xFP16 operand split
-        # instead of 3xTF32; 0 = fp32 FFMA kernels.  Names: 'fp32' (0), '3xtf32' (7), '3xfp16' (15).
+        # instead of 3xTF32, 16 (with 8) = the single fp16 product x_hi.w_hi (fp16-grade accuracy, faster sampling);
+        # 0 = fp32 FFMA kernels.  Names: 'fp32' (0), '3xtf32' (7), '3xfp16' (15), '1xfp16' (31).
         # 'auto' = '3xfp16' when hidden_nf is 128, 192 or 256 (the widths with tensor-core kernels), else 'fp32'.
         self._math_mode = os.environ.get('DSB_MATH_MODE', 'auto')
         # fixed-order receiver sums (bit-identical repeat of a call, see include/diffsbdd_b200.h): True | False | 'auto'
@@ -201,6 +202,8 @@ class EGNNDynamics(nn.Module):
             return 7
         if m == '3xfp16':
             return 15
+        if m == '1xfp16':
+            return 31
         return int(m)
 
     @math_mode.setter

@@ -169,7 +169,12 @@ int dsb_set_programmatic_launch(int enable);
  * 8 selects the operand format of those kernels: 0 = 3xTF32 (tf32 operands, 8-bit exponent, any range),
  * 8 = 3xFP16 (f16 operands: half the shared-memory operand traffic, twice the MMA rate; weights are pre-scaled per matrix
  * with an exact power of two; an activation beyond the fp16 range turns into NaN at the output and raises through
- * status[0]).  0 = fp32 FFMA kernels everywhere.  Only hidden_nf 128, 192 and 256 have tensor-core kernels. */
+ * status[0]).  16, valid only together with 8, = single product: x.w ~= x_hi.w_hi, the fp16 operands of the 3xFP16 split
+ * without their residuals, accumulated in fp32 (a third of the wgmmas, half the operand stores and weight-stream bytes).
+ * Its accuracy is fp16-grade, not fp32-grade: each operand carries a relative rounding error up to 2^-11, so a contraction
+ * is off by up to ~2^-10 sum|x||w| and results are well outside the fp32 parity tolerance; its range limit is that of
+ * 3xFP16.  Bit 16 without bit 8 returns DSB_ERR_INVALID_ARGUMENT.  0 = fp32 FFMA kernels everywhere.  Only hidden_nf
+ * 128, 192 and 256 have tensor-core kernels. */
 int dsb_dynamics_set_math_mode(dsb_dynamics* dyn, int mode);
 
 /* ---- deterministic mode (per module; default off).  enable: 1 on, 0 off, negative = query only.  Returns the previous
