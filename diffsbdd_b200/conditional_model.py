@@ -25,7 +25,8 @@ import torch.nn.functional as F
 
 from . import _native, seeded
 from .dynamics import EGNNDynamics
-from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_add, scatter_mean, num_nodes_to_batch_mask
+from .en_diffusion import (EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, scatter_add, scatter_mean,
+                           num_nodes_to_batch_mask)
 
 
 class ConditionalDDPM(EnVariationalDiffusion):
@@ -133,15 +134,15 @@ class ConditionalDDPM(EnVariationalDiffusion):
         inp = [self.alpha(gamma_s, s_arr), self.sigma(gamma_s, s_arr), alpha_ts, sigma_ts]
         return t_arr.float().contiguous(), torch.cat([a, c, sg] + inp, dim=1).float().contiguous()
 
-    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, seeds=None):
+    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, seeds=None, sampler='ddpm', eta=0.0):
         """Static buffers + captured graphs for one batch layout.  A cached engine is reused only while everything a
         captured graph bakes in is unchanged: batch layout (mask contents), the native module generation (packed-weight
-        blob), its arithmetic mode and its workspace/status buffers, and whether its noise is seeded (the seeds themselves
-        are a static buffer, refreshed on every call)."""
+        blob), its arithmetic mode and its workspace/status buffers, whether its noise is seeded (the seeds themselves
+        are a static buffer, refreshed on every call), and the sampler with its eta."""
         device = z_lig.device
         dyn: EGNNDynamics = self.dynamics
         dyn._ensure_handle(device)
-        key = (tuple(z_lig.shape), tuple(xh_pocket.shape), n_samples, timesteps, str(device), seeds is not None)
+        key = (tuple(z_lig.shape), tuple(xh_pocket.shape), n_samples, timesteps, str(device), seeds is not None, sampler, eta)
         st = self._graph_cache.get(key)
         if st is not None:
             same_layout = torch.equal(st['lig_mask'], lig_mask) and torch.equal(st['pocket_mask'], pocket_mask)
@@ -163,6 +164,12 @@ class ConditionalDDPM(EnVariationalDiffusion):
             if seeds is not None:     # seeds, draw ids of the step's three draws, resampling round u
                 st.update(seeds=torch.empty_like(seeds), draw=torch.zeros(3, dtype=torch.int64, device=device),
                           u=torch.zeros(1, dtype=torch.int64, device=device))
+            if sampler != 'ddpm':     # few-step samplers: their coefficient table; DDIM at eta = 0 adds 0 * (zeroed noise)
+                _, fast = self._fast_tables(timesteps, sampler, eta, device)
+                st.update(fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device), eta=eta)
+                st['noise'].zero_()
+                if sampler == 'dpmpp_2m':
+                    st['hist'] = torch.zeros_like(z_lig)
             self._graph_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -172,7 +179,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def _captured_step(self, st, kind):
         """One iteration as a python callable over the static buffers of ``st``.
         kind: 'reverse' (z_t -> z_s, step -= 1) | 'inpaint_renoise' (reverse step + RePaint blend + re-noise to t) |
-        'inpaint_last' (reverse step + blend, step -= 1)."""
+        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' (_fast_captured_step)."""
+        if kind in ('ddim', 'dpmpp_2m'):
+            return self._fast_captured_step(st, kind)
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
@@ -230,6 +239,8 @@ class ConditionalDDPM(EnVariationalDiffusion):
         st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
         if st['seeded']:
             st['u'].zero_()
+        if 'hist' in st:
+            st['hist'].zero_()
 
     def _graph(self, st, kind, z_lig, xh_pocket, first_s):
         """Captured CUDA graph of ``kind`` (captured on first use; capture leaves the static state as it found it)."""
@@ -282,6 +293,90 @@ class ConditionalDDPM(EnVariationalDiffusion):
         dyn.check_status()
         return st['z'].clone(), st['pocket'].clone()
 
+    def _fast_captured_step(self, st, kind):
+        """One 'ddim' or 'dpmpp_2m' step over the static buffers of ``st`` (step -= 1): table row of the step counter ->
+        native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0) or
+        dsb_ddpm_multistep_update."""
+        dyn: EGNNDynamics = self.dynamics
+        lib = _native.load()
+        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
+        NL, NP = st['z'].shape[0], st['pocket'].shape[0]
+        k = st['fast_table'].shape[1]
+
+        def run():
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            idx = st['step'].clamp(min=0)
+            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
+            st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, k))
+            eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
+            if kind == 'ddim':
+                if st['eta'] > 0 and st['seeded']:
+                    seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
+                    seeded.fill(st['noise'], _native.RNG_LIGAND, st['seeds'],
+                                st['draw'][seeded.PURPOSE_REVERSE:seeded.PURPOSE_REVERSE + 1], lm, pm)
+                elif st['eta'] > 0:
+                    st['noise'].normal_()
+                _native.check(lib.dsb_ddpm_ligand_update(
+                    st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef_fast'].data_ptr(), lm.data_ptr(),
+                    pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, st['z'].data_ptr(),
+                    st['pocket'].data_ptr(), stream))
+            else:
+                _native.check(lib.dsb_ddpm_multistep_update(
+                    st['z'].data_ptr(), st['pocket'].data_ptr(), st['hist'].data_ptr(), None, eps.data_ptr(), None,
+                    st['coef_fast'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, 0,
+                    stream))
+            st['step'].sub_(1)
+        return run
+
+    def _graphed_fast_loop(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta, return_frames,
+                           out_lig, out_pocket):
+        """The whole 'ddim' / 'dpmpp_2m' reverse loop as ``timesteps`` replays of one captured step; frames are copied from
+        the static state between replays, so the history of the multistep sampler runs through them."""
+        dyn: EGNNDynamics = self.dynamics
+        st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, self._seeds(), sampler, eta)
+        s0 = timesteps - 1
+        prev_defer = dyn.defer_status_check
+        dyn.defer_status_check = True
+        try:
+            g = self._graph(st, sampler, z_lig, xh_pocket, s0)
+            self._start(st, z_lig, xh_pocket, s0)
+            for s in reversed(range(timesteps)):
+                g.replay()
+                if (s * return_frames) % timesteps == 0:
+                    idx = (s * return_frames) // timesteps
+                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(st['z'], st['pocket'])
+        finally:
+            dyn.defer_status_check = prev_defer
+        dyn.check_status()
+        return st['z'].clone(), st['pocket'].clone()
+
+    def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta):
+        """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s (DESIGN §13); ``row`` [1, k]: the step's row of _fast_tables.  Returns
+        (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M only), in the frame of the returned z."""
+        nd = self.n_dims
+        c = row.expand(t.shape[0], -1)
+        cl = c[lig_mask]
+        eps, _ = self.dynamics(z_lig, xh_pocket, t, lig_mask, pocket_mask)
+        if sampler == 'ddim':
+            mu = z_lig / cl[:, 0:1] - cl[:, 1:2] * eps
+            if eta > 0:
+                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
+                z_lig, xh_pocket = self.sample_normal_zero_com(mu, xh_pocket, c[:, 2:3], lig_mask, pocket_mask)
+            else:
+                xh_pocket = xh_pocket.clone()
+                mu[:, :nd], xh_pocket[:, :nd] = self.remove_mean_batch(mu[:, :nd], xh_pocket[:, :nd], lig_mask, pocket_mask)
+                z_lig = mu
+            return z_lig, xh_pocket, hist
+        x0 = (z_lig - cl[:, 3:4] * eps) * cl[:, 2:3]
+        z_lig = cl[:, 0:1] * z_lig + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0 - cl[:, 4:5] * hist)
+        # the ligand COM leaves z, the pocket and the history together (one mean, subtracted from both)
+        NP = xh_pocket.shape[0]
+        xh_pocket = xh_pocket.clone()
+        z_lig[:, :nd], moved = self.remove_mean_batch(z_lig[:, :nd], torch.cat((xh_pocket[:, :nd], x0[:, :nd])), lig_mask,
+                                                      torch.cat((pocket_mask, lig_mask)))
+        xh_pocket[:, :nd], x0[:, :nd] = moved[:NP], moved[NP:]
+        return z_lig, xh_pocket, x0
+
     def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,
                               timesteps, resamplings, return_frames, out_lig, out_pocket):
         """The double loop of conditional_model.py:616-674 as graph replays: per (s, u) one captured graph = native
@@ -316,9 +411,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
     # ---- public samplers ------------------------------------------------------------------------------------
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None):
+    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None, sampler='ddpm', eta=0.0):
         """conditional_model.py:479-555.  ``seeds``: one int64 per sample (seeded.py); every draw then comes from the
-        sample's own seed instead of torch's global generator."""
+        sample's own seed instead of torch's global generator.  ``sampler``: 'ddpm' (the reference's ancestral step),
+        'ddim' (with noise level ``eta`` in [0, 1]) or 'dpmpp_2m', on the same ``timesteps`` grid (DESIGN §13)."""
+        check_sampler(sampler, eta)
         timesteps = self.T if timesteps is None else timesteps
         assert 0 < return_frames <= timesteps
         assert timesteps % return_frames == 0
@@ -327,9 +424,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
         seeds = seeded.as_seeds(seeds, n_samples, device)
         lig_mask = num_nodes_to_batch_mask(n_samples, num_nodes_lig, device)
         with self._seeded(seeds, lig_mask, pocket['mask']):
-            return self._sample_given_pocket(pocket, lig_mask, n_samples, return_frames, timesteps)
+            return self._sample_given_pocket(pocket, lig_mask, n_samples, return_frames, timesteps, sampler, float(eta))
 
-    def _sample_given_pocket(self, pocket, lig_mask, n_samples, return_frames, timesteps):
+    def _sample_given_pocket(self, pocket, lig_mask, n_samples, return_frames, timesteps, sampler='ddpm', eta=0.0):
         if self._rng is not None:
             seeded.check_schedule(timesteps)
         device = pocket['x'].device
@@ -348,7 +445,21 @@ class ConditionalDDPM(EnVariationalDiffusion):
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + xh_pocket.size(), device=device)
 
-        if self._use_graph(device):
+        if sampler != 'ddpm' and self._use_graph(device):
+            z_lig, xh_pocket = self._graphed_fast_loop(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples, timesteps, sampler,
+                                                       eta, return_frames, out_lig, out_pocket)
+            self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
+        elif sampler != 'ddpm':
+            t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
+            hist = torch.zeros_like(z_lig)
+            for s in reversed(range(0, timesteps)):
+                z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
+                                                         hist, lig_mask, pocket['mask'], sampler, eta)
+                if (s * return_frames) % timesteps == 0:
+                    idx = (s * return_frames) // timesteps
+                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
+            self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
+        elif self._use_graph(device):
             stride = timesteps // return_frames       # frames are saved at s = idx * stride
             s_hi = timesteps - 1
             while s_hi >= 0:
@@ -642,7 +753,8 @@ class SimpleConditionalDDPM(ConditionalDDPM):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None):
+    def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None, sampler='ddpm', eta=0.0):
+        check_sampler(sampler, eta)
         pocket_com = scatter_mean(pocket['x'], pocket['mask'], dim=0)
         pocket['x'] = pocket['x'] - pocket_com[pocket['mask']]
-        return super().sample_given_pocket(pocket, num_nodes_lig, return_frames, timesteps, seeds)
+        return super().sample_given_pocket(pocket, num_nodes_lig, return_frames, timesteps, seeds, sampler, eta)

@@ -651,6 +651,62 @@ __global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
   }
 }
 
+
+// ---- DPM-Solver++(2M) step of both models (the contract is in include/diffsbdd_b200.h) ---------------------------------
+// One element of the step: x0 = (z - sigma_t eps) * inv_alpha_t ; D = (1 + w) x0 - w hist (x0 alone when w = 0, so the
+// history is not read on a first step) ; z' = c0 z + c1 D.  Writes z' and x0 in place; returns z'.
+__device__ __forceinline__ float multistep_elem(float* z, float* hist, const float* __restrict__ eps, size_t idx, float c0,
+                                                float c1, float inv_alpha, float sigma, float w) {
+  const float x0 = (z[idx] - sigma * eps[idx]) * inv_alpha;
+  const float d = w != 0.f ? (1.f + w) * x0 - w * hist[idx] : x0;
+  const float v = c0 * z[idx] + c1 * d;
+  z[idx] = v;
+  hist[idx] = x0;
+  return v;
+}
+
+// One block per graph; the COM of z'.x (ligand only, or ligand + pocket when `joint`) is summed in a fixed order and
+// removed from z', from the pocket coordinates and from the history written by this step.
+__global__ void __launch_bounds__(128) ddpm_multistep_kernel(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
+                                                              const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
+                                                              const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms,
+                                                              const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R,
+                                                              int joint) {
+  const int g = blockIdx.x;
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
+  const int D = 3 + A, DR = 3 + R;
+  const float c0 = coef[g * 5 + 0], c1 = coef[g * 5 + 1], inv_alpha = coef[g * 5 + 2], sigma = coef[g * 5 + 3],
+              w = coef[g * 5 + 4];
+  __shared__ float red[9][4];
+  float s[3] = {0.f, 0.f, 0.f};
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const float v = multistep_elem(z_lig, h_lig, eps_lig, (size_t)idx, c0, c1, inv_alpha, sigma, w);
+    const int c = idx % D;
+    if (c < 3) s[c] += v;
+  }
+  if (joint) {
+    for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+      const float v = multistep_elem(z_poc, h_poc, eps_poc, (size_t)idx, c0, c1, inv_alpha, sigma, w);
+      const int c = idx % DR;
+      if (c < 3) s[c] += v;
+    }
+  }
+  block_sum(s, 3, red);
+  const float cnt = joint ? sp.n : ((sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f);
+  const float m0 = s[0] / cnt, m1 = s[1] / cnt, m2 = s[2] / cnt;
+  __syncthreads();
+  for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
+    const size_t r = (size_t)i * D;
+    z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
+    h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
+  }
+  for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
+    const size_t r = (size_t)i * DR;
+    z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
+    if (joint) { h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2; }
+  }
+}
+
 // ---- seeded per-graph random numbers (dsb_seeded_normal; the contract is in include/diffsbdd_b200.h) -------------------
 // Philox4x32-10 (Salmon et al., SC'11): 10 rounds, the key bumped by the Weyl constants between rounds.
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
@@ -1176,6 +1232,23 @@ int dsb_ddpm_joint_update(float* z_lig, float* z_pocket, const float* eps_lig, c
   ddpm_joint_update_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(z_lig, z_pocket, eps_lig, eps_pocket, noise_x, noise_h_lig,
                                                                                 noise_h_pocket, coef, mask_atoms, mask_residues,
                                                                                 (int)n_atoms, (int)n_residues, atom_nf, residue_nf);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_multistep_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
+                              const float* eps_pocket, const float* coef, const int64_t* mask_atoms,
+                              const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                              int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!z_lig || !hist_lig || !eps_lig || !coef || !mask_atoms || (n_residues > 0 && (!z_pocket || !mask_residues)) ||
+      (joint && n_residues > 0 && (!hist_pocket || !eps_pocket))) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  ddpm_multistep_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(z_lig, z_pocket, hist_lig, hist_pocket, eps_lig,
+                                                                             eps_pocket, coef, mask_atoms, mask_residues,
+                                                                             (int)n_atoms, (int)n_residues, atom_nf, residue_nf,
+                                                                             joint != 0);
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }

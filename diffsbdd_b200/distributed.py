@@ -12,6 +12,8 @@ from typing import Dict, List, Tuple
 import torch
 import torch.distributed as dist
 
+from .en_diffusion import check_sampler
+
 
 def shard_bounds(n_items: int, world_size: int, rank: int) -> Tuple[int, int]:
     """Contiguous split of ``n_items`` pockets; the first ``n_items % world_size`` ranks get one extra."""
@@ -38,7 +40,7 @@ def shard_seeds(seeds, lo: int, hi: int) -> torch.Tensor:
 
 @torch.no_grad()
 def sample_given_pocket_sharded(ddpm, pocket: Dict[str, torch.Tensor], num_nodes_lig: torch.Tensor, base_seed: int = 0,
-                                timesteps=None, group=None, seeds=None):
+                                timesteps=None, group=None, seeds=None, sampler='ddpm', eta=0.0):
     """Runs ``ddpm.sample_given_pocket`` on this rank's shard of the pockets and gathers the ligands of all ranks.
 
     ``pocket``/``num_nodes_lig`` describe the WHOLE job on every rank (device tensors of this rank).  Returns
@@ -47,8 +49,10 @@ def sample_given_pocket_sharded(ddpm, pocket: Dict[str, torch.Tensor], num_nodes
 
     ``seeds`` (one int64 per pocket of the whole job): rank r samples its pockets with ``seeds[lo:hi]`` and ``base_seed`` is
     ignored, so in deterministic mode the gathered ligands are the same for any number of ranks.  Without ``seeds`` every
-    rank draws from torch's generator seeded with ``base_seed + rank``.
+    rank draws from torch's generator seeded with ``base_seed + rank``.  ``sampler`` / ``eta``: as
+    ``ConditionalDDPM.sample_given_pocket``.
     """
+    check_sampler(sampler, eta)
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     rank = dist.get_rank(group) if dist.is_initialized() else 0
     n = len(pocket['size'])
@@ -65,8 +69,10 @@ def sample_given_pocket_sharded(ddpm, pocket: Dict[str, torch.Tensor], num_nodes
         if dev.type == 'cuda':
             torch.cuda.manual_seed(base_seed + rank)
     if hi > lo:
-        local = ddpm.sample_given_pocket(shard_pocket(pocket, lo, hi), num_nodes_lig[lo:hi], timesteps=timesteps,
-                                         **({} if local_seeds is None else {'seeds': local_seeds}))
+        extra = {} if local_seeds is None else {'seeds': local_seeds}
+        if sampler != 'ddpm':
+            extra.update(sampler=sampler, eta=eta)
+        local = ddpm.sample_given_pocket(shard_pocket(pocket, lo, hi), num_nodes_lig[lo:hi], timesteps=timesteps, **extra)
     else:
         width = ddpm.n_dims + ddpm.atom_nf
         local = (torch.zeros((0, width), device=dev), torch.zeros((0, ddpm.n_dims + ddpm.residue_nf), device=dev),

@@ -116,6 +116,51 @@ def cosine_alphas2(timesteps: int, s: float = 0.008):
     return np.cumprod(1.0 - betas)
 
 
+# ---- few-step samplers (DESIGN §13) --------------------------------------------------------------------------------------
+SAMPLERS = ('ddpm', 'ddim', 'dpmpp_2m')
+
+
+def check_sampler(sampler, eta):
+    """Raises ValueError unless ``sampler`` is one of SAMPLERS, eta lies in [0, 1], and eta is 0 for every sampler but 'ddim'."""
+    if sampler not in SAMPLERS:
+        raise ValueError(f"unknown sampler {sampler!r}: expected one of {', '.join(SAMPLERS)}")
+    if not 0.0 <= float(eta) <= 1.0:
+        raise ValueError(f'eta must lie in [0, 1], got {eta}')
+    if float(eta) != 0.0 and sampler != 'ddim':
+        raise ValueError(f"eta = {eta} needs sampler='ddim' ({sampler!r} is deterministic)")
+
+
+def fast_coefficients(gamma_s, gamma_t, sampler, eta=0.0):
+    """float64 per-step coefficients of the 'ddim' and 'dpmpp_2m' steps from gamma at s and t ([N, 1] each, row k = step
+    s = k, so that row k + 1 is the step run just before row k).  With alpha^2 = sigmoid(-gamma), sigma^2 = sigmoid(gamma):
+
+    'ddim'     (alpha_{t|s}, alpha_s sigma_t / alpha_t - sqrt(sigma_s^2 - eta^2 st^2), eta st), st = sigma_{t|s} sigma_s / sigma_t:
+               the (c0, c1, c2) of z / c0 - c1 eps_hat + c2 noise.  c1 is evaluated as (sigma^2_{t|s} / alpha^2_{t|s} +
+               eta^2 st^2) / (sigma_t / alpha_{t|s} + sqrt(sigma_s^2 - eta^2 st^2)), the same number without the cancellation
+               of the difference, so that at eta = 1 it is the ancestral sigma^2_{t|s} / (alpha_{t|s} sigma_t) to rounding.
+    'dpmpp_2m' (sigma_s / sigma_t, -alpha_s (e^-h - 1), 1 / alpha_t, sigma_t, w), h = lambda_s - lambda_t, lambda = -gamma / 2,
+               w = h / (2 h_prev) with h_prev the h of row k + 1, and w = 0 in the last row (the first step run)."""
+    gs, gt = gamma_s.detach().double(), gamma_t.detach().double()
+    s2_s, s2_t = torch.sigmoid(gs), torch.sigmoid(gt)
+    alpha_s, alpha_t = torch.sqrt(torch.sigmoid(-gs)), torch.sqrt(torch.sigmoid(-gt))
+    sigma_s, sigma_t = torch.sqrt(s2_s), torch.sqrt(s2_t)
+    if sampler == 'ddim':
+        eta2 = float(eta) ** 2
+        sigma2_ts = -torch.expm1(F.softplus(gs) - F.softplus(gt))
+        alpha_ts = torch.exp(0.5 * (F.logsigmoid(-gt) - F.logsigmoid(-gs)))
+        tilde2 = sigma2_ts * s2_s / s2_t
+        # sigma_s^2 - eta^2 tilde^2 = sigma_s^2 (alpha_ts^2 sigma_s^2 + (1 - eta^2) sigma2_ts) / sigma_t^2, a sum of non-negatives
+        keep = torch.sqrt(s2_s * (alpha_ts ** 2 * s2_s + (1.0 - eta2) * sigma2_ts) / s2_t)
+        c1 = (sigma2_ts / alpha_ts ** 2 + eta2 * tilde2) / (sigma_t / alpha_ts + keep)
+        return torch.cat([alpha_ts, c1, float(eta) * torch.sqrt(tilde2)], dim=1)
+    if sampler == 'dpmpp_2m':
+        h = 0.5 * (gt - gs)
+        w = torch.zeros_like(h)
+        w[:-1] = h[:-1] / (2.0 * h[1:])
+        return torch.cat([sigma_s / sigma_t, -alpha_s * torch.expm1(-h), 1.0 / alpha_t, sigma_t, w], dim=1)
+    raise ValueError(sampler)
+
+
 class PredefinedNoiseSchedule(nn.Module):
     """Lookup table gamma[t_int] = -(log alpha^2 - log sigma^2) (en_diffusion.py:1158-1190)."""
 
@@ -471,12 +516,21 @@ class EnVariationalDiffusion(nn.Module):
         inp = [self.alpha(gamma_s, s_arr), self.sigma(gamma_s, s_arr), alp_j, sig_j]
         return t_arr.float().contiguous(), torch.cat(rev + inp, dim=1).float().contiguous()
 
-    def _joint_engine(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, jump_length):
+    def _fast_tables(self, timesteps, sampler, eta, device):
+        """Per-step t and coefficients of the 'ddim' / 'dpmpp_2m' steps s = 0..timesteps-1 (t = s+1) for both engines:
+        fast_coefficients in float64 from the fp32 gamma values, cast to fp32, so that eager and graph steps use the same bits."""
+        s_int = torch.arange(timesteps, device=device).view(-1, 1)
+        t_arr, s_arr = (s_int + 1) / timesteps, s_int / timesteps
+        coef = fast_coefficients(self.gamma(s_arr), self.gamma(t_arr), sampler, eta)
+        return t_arr.float().contiguous(), coef.float().contiguous()
+
+    def _joint_engine(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, jump_length, sampler='ddpm', eta=0.0):
         dyn = self.dynamics
         device = z_lig.device
         dyn._ensure_handle(device)
         seeds = self._seeds()
-        key = (tuple(z_lig.shape), tuple(z_pocket.shape), n_samples, timesteps, jump_length, str(device), seeds is not None)
+        key = (tuple(z_lig.shape), tuple(z_pocket.shape), n_samples, timesteps, jump_length, str(device), seeds is not None,
+               sampler, eta)
         st = self._joint_cache.get(key)
         if st is not None:
             same = torch.equal(st['lig_mask'], lig_mask) and torch.equal(st['pocket_mask'], pocket_mask)
@@ -496,6 +550,13 @@ class EnVariationalDiffusion(nn.Module):
             if seeds is not None:     # seeds, draw ids of the step's three draws, jumps back so far u
                 st.update(seeds=torch.empty_like(seeds), draw=torch.zeros(3, dtype=torch.int64, device=device),
                           u=torch.zeros(1, dtype=torch.int64, device=device))
+            if sampler != 'ddpm':     # few-step samplers: their coefficient table; DDIM at eta = 0 adds 0 * (zeroed noise)
+                _, fast = self._fast_tables(timesteps, sampler, eta, device)
+                st.update(fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device), eta=eta)
+                for x in st['n_rev']:
+                    x.zero_()
+                if sampler == 'dpmpp_2m':
+                    st['hist'] = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket))
             self._joint_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -504,9 +565,12 @@ class EnVariationalDiffusion(nn.Module):
 
     def _joint_step(self, st, kind):
         """kind: 'reverse' (sample: one joint reverse step, step -= 1) | 'inpaint' (noised known part + reverse step + blend,
-        step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1)."""
+        step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1) | 'ddim' | 'dpmpp_2m'
+        (_joint_fast_captured_step)."""
         import ctypes as C
         from . import _native, seeded
+        if kind in ('ddim', 'dpmpp_2m'):
+            return self._joint_fast_captured_step(st, kind)
         dyn, lib = self.dynamics, _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
         NL, NP = st['zl'].shape[0], st['zp'].shape[0]
@@ -562,6 +626,8 @@ class EnVariationalDiffusion(nn.Module):
         st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
         if st['seeded']:
             st['u'].zero_()
+        for x in st.get('hist', ()):
+            x.zero_()
 
     def _joint_graph(self, st, kind, z_lig, z_pocket, first_s):
         g = st['graphs'].get(kind)
@@ -609,19 +675,111 @@ class EnVariationalDiffusion(nn.Module):
         dyn.check_status()
         return st['zl'].clone(), st['zp'].clone()
 
+    def _joint_fast_captured_step(self, st, kind):
+        """One 'ddim' or 'dpmpp_2m' step of the joint model over the static buffers of ``st`` (step -= 1): table row of
+        the step counter -> native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients (noise drawn only at eta > 0)
+        or dsb_ddpm_multistep_update."""
+        import ctypes as C
+        from . import _native, seeded
+        dyn, lib = self.dynamics, _native.load()
+        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
+        NL, NP = st['zl'].shape[0], st['zp'].shape[0]
+        ptr = lambda x: x.data_ptr()
+        roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
+        k = st['fast_table'].shape[1]
+        rev = slice(seeded.PURPOSE_REVERSE, seeded.PURPOSE_REVERSE + 1)
+
+        def run():
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            idx = st['step'].clamp(min=0)
+            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
+            st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, k))
+            eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
+            if kind == 'ddim':
+                if st['eta'] > 0:
+                    if st['seeded']:
+                        seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
+                        for x, role in zip(st['n_rev'], roles):
+                            seeded.fill(x, role, st['seeds'], st['draw'][rev], lm, pm)
+                    else:
+                        for x in st['n_rev']:
+                            x.normal_()
+                nx, nhl, nhp = st['n_rev']
+                _native.check(lib.dsb_ddpm_joint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
+                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
+            else:
+                hl, hp = st['hist']
+                _native.check(lib.dsb_ddpm_multistep_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(st['coef_fast']), ptr(lm),
+                    ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, stream))
+            st['step'].sub_(1)
+        return run
+
+    def _graphed_joint_fast_loop(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta,
+                                 return_frames, out_lig, out_pocket):
+        """The whole 'ddim' / 'dpmpp_2m' reverse loop as ``timesteps`` replays of one captured step; frames are copied from
+        the static state between replays, so the history of the multistep sampler runs through them."""
+        dyn = self.dynamics
+        st = self._joint_engine(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, 1, sampler, eta)
+        s0 = timesteps - 1
+        prev_defer, dyn.defer_status_check = dyn.defer_status_check, True
+        try:
+            g = self._joint_graph(st, sampler, z_lig, z_pocket, s0)
+            self._joint_start(st, z_lig, z_pocket, s0)
+            for s in reversed(range(timesteps)):
+                g.replay()
+                if (s * return_frames) % timesteps == 0:
+                    idx = (s * return_frames) // timesteps
+                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(st['zl'], st['zp'])
+        finally:
+            dyn.defer_status_check = prev_defer
+        dyn.check_status()
+        return st['zl'].clone(), st['zp'].clone()
+
+    def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta):
+        """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s of the joint model (DESIGN §13); ``row`` [1, k]: the step's row of
+        _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step (2M only)."""
+        from . import seeded
+        nd = self.n_dims
+        c = row.expand(t.shape[0], -1)
+        cl, cp = c[lig_mask], c[pocket_mask]
+        eps_l, eps_p = self.dynamics(zl, zp, t, lig_mask, pocket_mask)
+        if sampler == 'ddim':
+            mu_l = zl / cl[:, 0:1] - cl[:, 1:2] * eps_l
+            mu_p = zp / cp[:, 0:1] - cp[:, 1:2] * eps_p
+            if eta > 0:
+                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
+                mu_l, mu_p = self.sample_normal(mu_l, mu_p, c[:, 2:3], lig_mask, pocket_mask)
+            zl, zp = self._project_joint_com(mu_l, mu_p, lig_mask, pocket_mask)
+            return zl, zp, hl, hp
+        x0_l = (zl - cl[:, 3:4] * eps_l) * cl[:, 2:3]
+        x0_p = (zp - cp[:, 3:4] * eps_p) * cp[:, 2:3]
+        zl = cl[:, 0:1] * zl + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0_l - cl[:, 4:5] * hl)
+        zp = cp[:, 0:1] * zp + cp[:, 1:2] * ((1 + cp[:, 4:5]) * x0_p - cp[:, 4:5] * hp)
+        mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lig_mask, pocket_mask)), dim=0,
+                            dim_size=t.shape[0])
+        for x, m in ((zl, lig_mask), (zp, pocket_mask), (x0_l, lig_mask), (x0_p, pocket_mask)):
+            x[:, :nd] -= mean[m]
+        return zl, zp, x0_l, x0_p
+
     @follows_dynamics_determinism
     @torch.no_grad()
-    def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu', seeds=None):
+    def sample(self, n_samples, num_nodes_lig, num_nodes_pocket, return_frames=1, timesteps=None, device='cpu', seeds=None,
+               sampler='ddpm', eta=0.0):
         """en_diffusion.py:581-651: unconditional joint sampling of ligand and pocket.  ``seeds``: one int64 per sample
-        (seeded.py); every draw then comes from the sample's own seed instead of torch's global generator."""
+        (seeded.py); every draw then comes from the sample's own seed instead of torch's global generator.  ``sampler``:
+        'ddpm' (the reference's ancestral step), 'ddim' (with noise level ``eta`` in [0, 1]) or 'dpmpp_2m', on the same
+        ``timesteps`` grid (DESIGN §13)."""
         from . import seeded
+        check_sampler(sampler, eta)
         seeds = seeded.as_seeds(seeds, n_samples, device)
         lig_mask = num_nodes_to_batch_mask(n_samples, num_nodes_lig, device)
         pocket_mask = num_nodes_to_batch_mask(n_samples, num_nodes_pocket, device)
         with self._seeded(seeds, lig_mask, pocket_mask):
-            return self._sample(n_samples, lig_mask, pocket_mask, return_frames, timesteps)
+            return self._sample(n_samples, lig_mask, pocket_mask, return_frames, timesteps, sampler, float(eta))
 
-    def _sample(self, n_samples, lig_mask, pocket_mask, return_frames, timesteps):
+    def _sample(self, n_samples, lig_mask, pocket_mask, return_frames, timesteps, sampler='ddpm', eta=0.0):
         from . import seeded
         timesteps = self.T if timesteps is None else timesteps
         assert 0 < return_frames <= timesteps and timesteps % return_frames == 0
@@ -633,7 +791,22 @@ class EnVariationalDiffusion(nn.Module):
         self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + z_pocket.size(), device=z_pocket.device)
-        if self._joint_use_graph(z_lig.device):
+        if sampler != 'ddpm' and self._joint_use_graph(z_lig.device):
+            z_lig, z_pocket = self._graphed_joint_fast_loop(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler,
+                                                            eta, return_frames, out_lig, out_pocket)
+            self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
+        elif sampler != 'ddpm':
+            t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
+            h_lig, h_pocket = torch.zeros_like(z_lig), torch.zeros_like(z_pocket)
+            for s in reversed(range(0, timesteps)):
+                z_lig, z_pocket, h_lig, h_pocket = self._joint_fast_step(
+                    s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, z_pocket, h_lig, h_pocket, lig_mask, pocket_mask,
+                    sampler, eta)
+                if (s * return_frames) % timesteps == 0:
+                    idx = (s * return_frames) // timesteps
+                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
+            self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
+        elif self._joint_use_graph(z_lig.device):
             stride = timesteps // return_frames       # frames are saved at s = idx * stride
             s_hi = timesteps - 1
             while s_hi >= 0:

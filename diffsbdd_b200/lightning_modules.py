@@ -25,7 +25,7 @@ import torch.nn.functional as F
 from . import seeded
 from .conditional_model import ConditionalDDPM, SimpleConditionalDDPM
 from .dynamics import EGNNDynamics
-from .en_diffusion import EnVariationalDiffusion, follows_dynamics_determinism, scatter_mean, num_nodes_to_batch_mask
+from .en_diffusion import EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, scatter_mean, num_nodes_to_batch_mask
 
 try:  # pragma: no cover - not installed in the offline image
     import pytorch_lightning as pl
@@ -172,11 +172,17 @@ class LigandPocketDDPM(_Base):
     @follows_dynamics_determinism
     @torch.no_grad()
     def generate_ligand_tensors(self, pocket, num_nodes_lig=None, timesteps=None, n_nodes_bias=0, n_nodes_min=0,
-                                seeds=None, **kwargs):
+                                seeds=None, sampler='ddpm', eta=0.0, **kwargs):
         """Everything ``generate_ligands`` does between pocket preparation and molecule building
         (lightning_modules.py:785-852): returns (xh_lig, xh_pocket, lig_mask, pocket_mask) in the original
         pocket frame.  ``seeds``: one int64 per sample (seeded.py); the ligand size prior and every sampler draw then come
-        from the sample's own seed (the size by inverse CDF over p(n_lig | n_pocket))."""
+        from the sample's own seed (the size by inverse CDF over p(n_lig | n_pocket)).  ``sampler`` / ``eta``: the reverse
+        step of ConditionalDDPM.sample_given_pocket; a joint model generates through RePaint inpainting, which has only
+        the 'ddpm' step."""
+        check_sampler(sampler, eta)
+        if sampler != 'ddpm' and type(self.ddpm) == EnVariationalDiffusion:
+            raise ValueError(f"sampler={sampler!r} is not supported for a joint model: it generates through RePaint inpainting, "
+                             f"which runs the 'ddpm' step only")
         self.ddpm.eval()
         seeds = seeded.as_seeds(seeds, len(pocket['size']), pocket['x'].device)
         pocket_com_before = scatter_mean(pocket['x'], pocket['mask'], dim=0)
@@ -197,7 +203,7 @@ class LigandPocketDDPM(_Base):
                 ligand, pocket, lig_fixed, pocket_fixed, timesteps=timesteps, seeds=seeds, **kwargs)
         elif type(self.ddpm) == ConditionalDDPM:
             xh_lig, xh_pocket, lig_mask, pocket_mask = self.ddpm.sample_given_pocket(
-                pocket, num_nodes_lig, timesteps=timesteps, seeds=seeds)
+                pocket, num_nodes_lig, timesteps=timesteps, seeds=seeds, sampler=sampler, eta=eta)
         else:
             raise NotImplementedError
         pocket_com_after = scatter_mean(xh_pocket[:, :self.x_dims], pocket_mask, dim=0)

@@ -260,6 +260,23 @@ int dsb_ddpm_joint_inpaint_update(float* z_lig, float* z_pocket, const float* xh
                                   int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf,
                                   void* stream);
 
+/* ---- DPM-Solver++(2M) step in data-prediction form (one launch, one block per graph; DESIGN §13), both models:
+ *   x0 = (z - sigma_t[g] eps_hat) * inv_alpha_t[g]                      (prediction of the clean sample)
+ *   D  = (1 + w[g]) x0 - w[g] hist ; D = x0 when w[g] == 0 (first step: hist is not read)
+ *   z' = c0[g] z + c1[g] D ;  hist' = x0
+ * then the COM of z'.x is removed from z'.x, from the pocket coordinates and from hist'.x:
+ *   joint == 0 (ConditionalDDPM): the LIGAND COM; the pocket (z_pocket) is only shifted; hist_pocket and eps_pocket are
+ *                                 not used and may be NULL.
+ *   joint != 0 (EnVariationalDiffusion): ligand AND pocket are updated and the COM is taken over ligand + pocket nodes.
+ * coef: device fp32 [n_graphs, 5] = (sigma_s/sigma_t, -alpha_s (e^-h - 1), 1/alpha_t, sigma_t, w) with h = lambda_s - lambda_t,
+ * lambda = -gamma/2, w = h / (2 h_prev) (0 on the first step).  hist_* [rows, 3 + nf]: x0 of the previous step in the current
+ * frame.  In place on z_lig, z_pocket, hist_lig, hist_pocket.  Masks sorted; each graph's sums run in a fixed order without
+ * atomics, so the result repeats bit for bit and a graph's result does not depend on the rest of its batch. */
+int dsb_ddpm_multistep_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
+                              const float* eps_pocket, const float* coef, const int64_t* mask_atoms,
+                              const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                              int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream);
+
 /* ---- evaluation-mode variational bound (validation / test NLL): what EnVariationalDiffusion.forward, ConditionalDDPM.forward
  * and SimpleConditionalDDPM.forward compute in eval mode besides the two denoiser calls and the per-graph scalar algebra.
  *
