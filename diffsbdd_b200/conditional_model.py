@@ -134,15 +134,19 @@ class ConditionalDDPM(EnVariationalDiffusion):
         inp = [self.alpha(gamma_s, s_arr), self.sigma(gamma_s, s_arr), alpha_ts, sigma_ts]
         return t_arr.float().contiguous(), torch.cat([a, c, sg] + inp, dim=1).float().contiguous()
 
-    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, seeds=None, sampler='ddpm', eta=0.0):
+    def _engine(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, seeds=None, sampler='ddpm', eta=0.0,
+                top=None):
         """Static buffers + captured graphs for one batch layout.  A cached engine is reused only while everything a
         captured graph bakes in is unchanged: batch layout (mask contents), the native module generation (packed-weight
         blob), its arithmetic mode and its workspace/status buffers, whether its noise is seeded (the seeds themselves
-        are a static buffer, refreshed on every call), and the sampler with its eta."""
+        are a static buffer, refreshed on every call), the sampler with its eta, and the top of its grid (``top``: as
+        _fast_tables; diversify's t*)."""
         device = z_lig.device
         dyn: EGNNDynamics = self.dynamics
         dyn._ensure_handle(device)
         key = (tuple(z_lig.shape), tuple(xh_pocket.shape), n_samples, timesteps, str(device), seeds is not None, sampler, eta)
+        if top is not None:
+            key += (top,)
         st = self._graph_cache.get(key)
         if st is not None:
             same_layout = torch.equal(st['lig_mask'], lig_mask) and torch.equal(st['pocket_mask'], pocket_mask)
@@ -165,11 +169,14 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 st.update(seeds=torch.empty_like(seeds), draw=torch.zeros(3, dtype=torch.int64, device=device),
                           u=torch.zeros(1, dtype=torch.int64, device=device))
             if sampler != 'ddpm':     # few-step samplers: their coefficient table; DDIM at eta = 0 adds 0 * (zeroed noise)
-                _, fast = self._fast_tables(timesteps, sampler, eta, device)
-                st.update(fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device), eta=eta)
+                fast_t, fast = self._fast_tables(timesteps, sampler, eta, device, top)
+                st.update(fast_t=fast_t, fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device),
+                          eta=eta, sampler=sampler)
                 st['noise'].zero_()
-                if sampler == 'dpmpp_2m':
+                if sampler == 'dpmpp_2m':   # RePaint rounds: the 2M row and the RePaint row in one [n, 9] buffer
                     st['hist'] = torch.zeros_like(z_lig)
+                    st.update(ms_table=torch.cat((fast, coef_table[:, 3:]), 1).contiguous(),
+                              coef9=torch.zeros((n_samples, 9), device=device))
             self._graph_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -179,9 +186,12 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def _captured_step(self, st, kind):
         """One iteration as a python callable over the static buffers of ``st``.
         kind: 'reverse' (z_t -> z_s, step -= 1) | 'inpaint_renoise' (reverse step + RePaint blend + re-noise to t) |
-        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' (_fast_captured_step)."""
+        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' (_fast_captured_step).  The inpainting kinds
+        of an engine built for a few-step sampler are _fast_inpaint_captured_step."""
         if kind in ('ddim', 'dpmpp_2m'):
             return self._fast_captured_step(st, kind)
+        if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
+            return self._fast_inpaint_captured_step(st, kind)
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
@@ -306,7 +316,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         def run():
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
             idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
+            st['t'].copy_(st['fast_t'].index_select(0, idx).expand(n, 1))
             st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, k))
             eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
             if kind == 'ddim':
@@ -329,11 +339,12 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return run
 
     def _graphed_fast_loop(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta, return_frames,
-                           out_lig, out_pocket):
+                           out_lig, out_pocket, top=None):
         """The whole 'ddim' / 'dpmpp_2m' reverse loop as ``timesteps`` replays of one captured step; frames are copied from
-        the static state between replays, so the history of the multistep sampler runs through them."""
+        the static state between replays, so the history of the multistep sampler runs through them.  ``top``: the grid's
+        top t as _fast_tables takes it (diversify)."""
         dyn: EGNNDynamics = self.dynamics
-        st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, self._seeds(), sampler, eta)
+        st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, self._seeds(), sampler, eta, top)
         s0 = timesteps - 1
         prev_defer = dyn.defer_status_check
         dyn.defer_status_check = True
@@ -350,9 +361,10 @@ class ConditionalDDPM(EnVariationalDiffusion):
         dyn.check_status()
         return st['z'].clone(), st['pocket'].clone()
 
-    def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta):
+    def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta, u=0):
         """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s (DESIGN §13); ``row`` [1, k]: the step's row of _fast_tables.  Returns
-        (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M only), in the frame of the returned z."""
+        (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M only), in the frame of the returned z.  ``u``: the
+        resampling round of the seeded DDIM draw (RePaint)."""
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
         cl = c[lig_mask]
@@ -360,7 +372,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         if sampler == 'ddim':
             mu = z_lig / cl[:, 0:1] - cl[:, 1:2] * eps
             if eta > 0:
-                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
+                self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
                 z_lig, xh_pocket = self.sample_normal_zero_com(mu, xh_pocket, c[:, 2:3], lig_mask, pocket_mask)
             else:
                 xh_pocket = xh_pocket.clone()
@@ -377,13 +389,115 @@ class ConditionalDDPM(EnVariationalDiffusion):
         xh_pocket[:, :nd], x0[:, :nd] = moved[:NP], moved[NP:]
         return z_lig, xh_pocket, x0
 
-    def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,
-                              timesteps, resamplings, return_frames, out_lig, out_pocket):
-        """The double loop of conditional_model.py:616-674 as graph replays: per (s, u) one captured graph = native
-        denoiser + fused reverse update + fused RePaint iteration (dsb_ddpm_inpaint_update); no torch op and no host
-        sync inside the loop."""
+    def _fast_inpaint_captured_step(self, st, kind):
+        """One RePaint round of an engine built for 'ddim' or 'dpmpp_2m' (DESIGN §14); kind as _captured_step
+        ('inpaint_renoise': re-noised, the round does not commit; 'inpaint_last': the last round of the step, which commits
+        its x0_hat as the 2M history).  DDIM: native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients ->
+        dsb_ddpm_inpaint_update.  2M: native denoiser -> dsb_ddpm_multistep_inpaint_update."""
         dyn: EGNNDynamics = self.dynamics
-        st = self._engine(z_lig, xh_pocket, lmask, pmask, n_samples, timesteps, self._seeds())
+        lib = _native.load()
+        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
+        NL, NP = st['z'].shape[0], st['pocket'].shape[0]
+        renoise = kind == 'inpaint_renoise'
+        ddim = st['sampler'] == 'ddim'
+
+        def draw(out, purpose):
+            if st['seeded']:
+                seeded.fill(out, _native.RNG_LIGAND, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
+            else:
+                out.normal_()
+
+        def run():
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            ptr = lambda x: x.data_ptr()
+            if st['seeded']:
+                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
+            idx = st['step'].clamp(min=0)
+            st['t'].copy_(st['fast_t'].index_select(0, idx).expand(n, 1))
+            if ddim:
+                st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
+                st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
+            else:
+                st['coef9'].copy_(st['ms_table'].index_select(0, idx).expand(n, 9))
+            eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
+            if ddim and st['eta'] > 0:
+                draw(st['noise'], seeded.PURPOSE_REVERSE)
+            draw(st['noise1'], seeded.PURPOSE_KNOWN)
+            if renoise:
+                draw(st['noise2'], seeded.PURPOSE_RENOISE)
+            ip = st['inpaint']
+            n2 = ptr(st['noise2']) if renoise else None
+            if ddim:
+                _native.check(lib.dsb_ddpm_ligand_update(
+                    ptr(st['z']), ptr(eps), ptr(st['noise']), ptr(st['coef_fast']), ptr(lm), ptr(pm), ptr(st['pocket']), NL, NP,
+                    n, self.atom_nf, self.residue_nf, ptr(st['z']), ptr(st['pocket']), stream))
+                _native.check(lib.dsb_ddpm_inpaint_update(
+                    ptr(st['z']), ptr(st['pocket']), ptr(ip['known']), ptr(ip['com0']), ptr(ip['fixed']), ptr(st['noise1']), n2,
+                    ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
+            else:
+                _native.check(lib.dsb_ddpm_multistep_inpaint_update(
+                    ptr(st['z']), ptr(st['pocket']), ptr(st['hist']), None, ptr(eps), None, ptr(ip['known']), None,
+                    ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None, ptr(st['coef9']),
+                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 0, int(not renoise), stream))
+            if renoise:
+                if st['seeded']:
+                    st['u'].add_(1)
+            else:
+                st['step'].sub_(1)
+                if st['seeded']:
+                    st['u'].zero_()
+        return run
+
+    def _fast_inpaint_step(self, s, u, t, row, gamma_s, gamma_t, z_lig, xh_pocket, hist, ligand_x, xh_ligand, com_pocket_0,
+                           lig_fixed, lmask, pmask, sampler, eta, last):
+        """Eager RePaint round (s, u) with the 'ddim' / 'dpmpp_2m' step (DESIGN §14): _inpaint's iteration with the few-step
+        step in place of the ancestral one; ``row`` [1, k]: the step's row of _fast_tables, ``last``: no re-noising after
+        this round.  2M: ``hist`` is x0_hat committed by the last round of step s + 1, kept in the pocket's frame: every
+        translation of the pocket coordinates moves it too, and the last round of step s commits its own x0_hat.  Returns
+        (z_lig, xh_pocket, hist)."""
+        nd, NL, NP = self.n_dims, z_lig.shape[0], xh_pocket.shape[0]
+        fixed_rows = lig_fixed.bool().view(-1)
+        if sampler == 'ddim':
+            z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u)
+            frame, fmask = xh_pocket[:, :nd], pmask
+        else:
+            c = row.expand(t.shape[0], -1)[lmask]
+            eps, _ = self.dynamics(z_lig, xh_pocket, t, lmask, pmask)
+            x0 = (z_lig - c[:, 3:4] * eps) * c[:, 2:3]
+            z_unknown = c[:, 0:1] * z_lig + c[:, 1:2] * ((1 + c[:, 4:5]) * x0 - c[:, 4:5] * hist)
+            # frame: the rows that every pocket translation moves (pocket, history, x0_hat), under the pocket's graph index
+            fmask = torch.cat((pmask, lmask, lmask))
+            z_unknown[:, :nd], frame = self.remove_mean_batch(
+                z_unknown[:, :nd], torch.cat((xh_pocket[:, :nd], hist[:, :nd], x0[:, :nd])), lmask, fmask)
+
+        # the rest is _inpaint's iteration, with ``frame`` in place of the pocket coordinates
+        com_pocket = scatter_mean(frame[:NP], pmask, dim=0)
+        xh_ligand[:, :nd] = ligand_x + (com_pocket - com_pocket_0)[lmask]
+        self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_KNOWN)
+        z_known, frame, _ = self.noised_representation(xh_ligand, frame, lmask, fmask, gamma_s)
+        com_noised = scatter_mean(z_known[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
+        com_denoised = scatter_mean(z_unknown[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
+        dx = com_denoised - com_noised
+        z_known[:, :nd] = z_known[:, :nd] + dx[lmask]
+        frame = frame + dx[fmask]
+        z_lig = z_known * lig_fixed + z_unknown * (1 - lig_fixed)
+        if not last:
+            self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_RENOISE)
+            z_lig, frame = self.sample_p_zt_given_zs(z_lig, frame, lmask, fmask, gamma_t, gamma_s)
+        xh_pocket = torch.cat((frame[:NP], xh_pocket[:, nd:]), dim=1)
+        if sampler == 'dpmpp_2m':
+            keep = x0 if last else hist
+            rows = frame[NP + NL:] if last else frame[NP:NP + NL]
+            hist = torch.cat((rows, keep[:, nd:]), dim=1)
+        return z_lig, xh_pocket, hist
+
+    def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,
+                              timesteps, resamplings, return_frames, out_lig, out_pocket, sampler='ddpm', eta=0.0):
+        """The double loop of conditional_model.py:616-674 as graph replays: per (s, u) one captured graph = native
+        denoiser + fused reverse update + fused RePaint iteration (dsb_ddpm_inpaint_update, or one
+        dsb_ddpm_multistep_inpaint_update under 2M); no torch op and no host sync inside the loop."""
+        dyn: EGNNDynamics = self.dynamics
+        st = self._engine(z_lig, xh_pocket, lmask, pmask, n_samples, timesteps, self._seeds(), sampler, eta)
         if st['inpaint'] is None:       # static buffers the captured RePaint iteration reads
             st['inpaint'] = dict(known=torch.empty_like(z_lig), com0=torch.empty_like(com_pocket_0, dtype=torch.float32),
                                  fixed=torch.empty(z_lig.shape[0], dtype=torch.float32, device=z_lig.device))
@@ -493,14 +607,20 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def inpaint(self, ligand, pocket, lig_fixed, resamplings=1, return_frames=1, timesteps=None, center='ligand', seeds=None):
+    def inpaint(self, ligand, pocket, lig_fixed, resamplings=1, return_frames=1, timesteps=None, center='ligand', seeds=None,
+                sampler='ddpm', eta=0.0):
         """conditional_model.py:558-686: RePaint-style conditional generation with fixed ligand atoms.  ``seeds``: as
-        sample_given_pocket."""
+        sample_given_pocket.  ``sampler`` / ``eta``: the reverse step of every RePaint round, as sample_given_pocket
+        (DESIGN §14)."""
+        self._check_fast_repaint(sampler, eta)
         seeds = seeded.as_seeds(seeds, len(ligand['size']), pocket['x'].device)
         with self._seeded(seeds, ligand['mask'], pocket['mask']):
-            return self._inpaint(ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center)
+            return self._inpaint(ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center, sampler, float(eta))
 
-    def _inpaint(self, ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center):
+    def _check_fast_repaint(self, sampler, eta):
+        check_sampler(sampler, eta)
+
+    def _inpaint(self, ligand, pocket, lig_fixed, resamplings, return_frames, timesteps, center, sampler='ddpm', eta=0.0):
         timesteps = self.T if timesteps is None else timesteps
         if self._rng is not None:
             seeded.check_schedule(timesteps, resamplings)
@@ -536,7 +656,23 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
         if use_graph:
             z_lig, xh_pocket = self._graphed_inpaint_loop(z_lig, xh_pocket, xh_ligand, com_pocket_0, lig_fixed, lmask, pmask,
-                                                         n_samples, timesteps, resamplings, return_frames, out_lig, out_pocket)
+                                                         n_samples, timesteps, resamplings, return_frames, out_lig, out_pocket,
+                                                         sampler, eta)
+        elif sampler != 'ddpm':
+            t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
+            hist = torch.zeros_like(z_lig)
+            for s in reversed(range(0, timesteps)):
+                for u in range(resamplings):
+                    s_array = torch.full((n_samples, 1), fill_value=s, device=device)
+                    t_array = (s_array + 1) / timesteps
+                    s_array = s_array / timesteps
+                    last = u == resamplings - 1
+                    z_lig, xh_pocket, hist = self._fast_inpaint_step(
+                        s, u, t_table[s].expand(n_samples, 1), coef[s:s + 1], self.gamma(s_array), self.gamma(t_array), z_lig,
+                        xh_pocket, hist, ligand['x'], xh_ligand, com_pocket_0, lig_fixed, lmask, pmask, sampler, eta, last)
+                    if last and (s * return_frames) % timesteps == 0:
+                        idx = (s * return_frames) // timesteps
+                        out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
         else:
             for s in reversed(range(0, timesteps)):
                 for u in range(resamplings):
@@ -688,14 +824,25 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
     @follows_dynamics_determinism
     @torch.no_grad()
-    def diversify(self, ligand, pocket, noising_steps, seeds=None):
+    def diversify(self, ligand, pocket, noising_steps, seeds=None, sampler='ddpm', eta=0.0, denoising_steps=None):
         """conditional_model.py:364-409: partially noise given ligands, then denoise them again.  ``seeds``: as
-        sample_given_pocket."""
+        sample_given_pocket.  ``sampler`` / ``eta``: the reverse step, as sample_given_pocket; ``denoising_steps``: the
+        number of reverse steps from t* = noising_steps / T down to 0 on the uniform grid t_k = k t* / denoising_steps,
+        1 <= denoising_steps <= noising_steps (None: noising_steps, the T grid; 'ddpm' runs the T grid only) (DESIGN §14)."""
+        self._check_fast_repaint(sampler, eta)
+        if denoising_steps is not None:
+            if int(denoising_steps) != denoising_steps or not 1 <= denoising_steps <= noising_steps:
+                raise ValueError(f'denoising_steps must be an integer in [1, noising_steps = {noising_steps}], '
+                                 f'got {denoising_steps}')
+            if sampler == 'ddpm' and denoising_steps != noising_steps:
+                raise ValueError(f"sampler='ddpm' denoises on the T grid: denoising_steps must be None or noising_steps "
+                                 f"({noising_steps}), got {denoising_steps}; use sampler='ddim' or 'dpmpp_2m' for fewer steps")
         seeds = seeded.as_seeds(seeds, len(pocket['size']), pocket['x'].device)
         with self._seeded(seeds, ligand['mask'], pocket['mask']):
-            return self._diversify(ligand, pocket, noising_steps)
+            return self._diversify(ligand, pocket, noising_steps, sampler, float(eta),
+                                   noising_steps if denoising_steps is None else int(denoising_steps))
 
-    def _diversify(self, ligand, pocket, noising_steps):
+    def _diversify(self, ligand, pocket, noising_steps, sampler='ddpm', eta=0.0, denoising_steps=None):
         if self._rng is not None:
             seeded.check_schedule(self.T)
         ligand, pocket = self.normalize(ligand, pocket)
@@ -705,7 +852,18 @@ class ConditionalDDPM(EnVariationalDiffusion):
         n_samples = len(pocket['size'])
         lig_mask = ligand['mask']
         self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
-        if self._use_graph(z_lig.device) and noising_steps > 0:
+        top = (noising_steps, timesteps)
+        if sampler != 'ddpm' and self._use_graph(z_lig.device) and noising_steps > 0:
+            frame = torch.empty((1,) + z_lig.shape, device=z_lig.device), torch.empty((1,) + xh_pocket.shape, device=z_lig.device)
+            z_lig, xh_pocket = self._graphed_fast_loop(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples, denoising_steps,
+                                                       sampler, eta, 1, *frame, top=top)
+        elif sampler != 'ddpm' and noising_steps > 0:
+            t_table, coef = self._fast_tables(denoising_steps, sampler, eta, z_lig.device, top)
+            hist = torch.zeros_like(z_lig)
+            for s in reversed(range(0, denoising_steps)):
+                z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
+                                                         hist, lig_mask, pocket['mask'], sampler, eta)
+        elif self._use_graph(z_lig.device) and noising_steps > 0:
             z_lig, xh_pocket = self._graphed_reverse_steps(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples,
                                                            noising_steps - 1, noising_steps, timesteps)
         else:
@@ -742,6 +900,11 @@ class SimpleConditionalDDPM(ConditionalDDPM):
     def _native_noise_conditional(self, xh_lig, eps, xh_pocket, lig_mask, pocket_mask, gamma):
         z_lig, _ = self._native_noise(xh_lig, eps, None, None, lig_mask, pocket_mask, gamma)   # no COM projection
         return z_lig, xh_pocket
+
+    def _check_fast_repaint(self, sampler, eta):
+        check_sampler(sampler, eta)
+        if sampler != 'ddpm':
+            raise ValueError(f"sampler={sampler!r}: inpaint and diversify of SimpleConditionalDDPM run the 'ddpm' step only")
 
     @follows_dynamics_determinism
     def forward(self, ligand, pocket, return_info=False):

@@ -707,6 +707,248 @@ __global__ void __launch_bounds__(128) ddpm_multistep_kernel(float* z_lig, float
   }
 }
 
+
+// ---- RePaint round with the DPM-Solver++(2M) step, both models (the contract is in include/diffsbdd_b200.h) -----------
+// The 2M part of one element: z' = c0 z + c1 D with D from x0 = (z - sigma_t eps) * inv_alpha_t and the history; x0 replaces
+// the history only when the round commits.  Returns z'.
+__device__ __forceinline__ float multistep_repaint_elem(float* z, float* hist, const float* __restrict__ eps, size_t idx,
+                                                        const float* k, int commit) {
+  const float x0 = (z[idx] - k[3] * eps[idx]) * k[2];
+  const float d = k[4] != 0.f ? (1.f + k[4]) * x0 - k[4] * hist[idx] : x0;
+  const float v = k[0] * z[idx] + k[1] * d;
+  z[idx] = v;
+  if (commit) hist[idx] = x0;
+  return v;
+}
+
+// Conditional model: the 2M step with its ligand-COM removal, then ddpm_inpaint_kernel's iteration on its output.  Every
+// translation of the pocket coordinates is applied to the history too, so that the history stays in the pocket's frame.
+__device__ __forceinline__ void multistep_repaint_cond(float* z, float* pocket, float* hist, const float* __restrict__ eps,
+                                                       const float* __restrict__ known, const float* __restrict__ com_pocket0,
+                                                       const float* __restrict__ fixed, const float* __restrict__ noise1,
+                                                       const float* __restrict__ noise2, const float* k, const JointSpan& sp,
+                                                       int A, int R, int commit, float (*red)[4]) {
+  const int g = blockIdx.x, l0 = sp.l0, l1 = sp.l1, p0 = sp.p0, p1 = sp.p1;
+  const int D = 3 + A, DR = 3 + R;
+  const float alpha_s = k[5], sigma_s = k[6], alpha_ts = k[7], sigma_ts = k[8];
+  const float nl = (l1 - l0) > 0 ? (float)(l1 - l0) : 1.f, np_ = (p1 - p0) > 0 ? (float)(p1 - p0) : 1.f;
+  float v[9] = {0.f, 0.f, 0.f};
+  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+    const float o = multistep_repaint_elem(z, hist, eps, (size_t)idx, k, commit);
+    const int c = idx % D;
+    if (c < 3) v[c] += o;
+  }
+  block_sum(v, 3, red);
+  const float m[3] = {v[0] / nl, v[1] / nl, v[2] / nl};
+  for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
+    const size_t r = (size_t)i * D;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { z[r + c] -= m[c]; hist[r + c] -= m[c]; }
+  }
+  for (int i = p0 + threadIdx.x; i < p1; i += blockDim.x) {
+    const size_t r = (size_t)i * DR;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) pocket[r + c] -= m[c];
+  }
+  __syncthreads();                      // z = z_unknown and the moved pocket are complete
+
+  // from here on ddpm_inpaint_kernel, with the history following the pocket
+  v[0] = v[1] = v[2] = 0.f;
+  for (int i = p0 + threadIdx.x; i < p1; i += blockDim.x) {
+    v[0] += pocket[(size_t)i * DR + 0]; v[1] += pocket[(size_t)i * DR + 1]; v[2] += pocket[(size_t)i * DR + 2];
+  }
+  block_sum(v, 3, red);
+  float shift[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) shift[c] = v[c] / np_ - com_pocket0[g * 3 + c];
+  auto zk_raw = [&](int idx, int c) {
+    const float xk = c < 3 ? known[idx] + shift[c] : known[idx];
+    return alpha_s * xk + sigma_s * noise1[idx];
+  };
+  v[0] = v[1] = v[2] = 0.f;
+  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+    const int c = idx % D;
+    if (c < 3) v[c] += zk_raw(idx, c);
+  }
+  block_sum(v, 3, red);
+  const float comk[3] = {v[0] / nl, v[1] / nl, v[2] / nl};
+  for (int q = 0; q < 7; ++q) v[q] = 0.f;
+  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+    const int c = idx % D, i = idx / D;
+    if (c < 3 && fixed[i] != 0.f) { v[c] += zk_raw(idx, c) - comk[c]; v[3 + c] += z[idx]; if (c == 0) v[6] += 1.f; }
+  }
+  block_sum(v, 7, red);
+  const float nf = v[6] > 0.f ? v[6] : 1.f;
+  float dx[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) dx[c] = v[3 + c] / nf - v[c] / nf;
+  float s2[3] = {0.f, 0.f, 0.f};
+  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+    const int c = idx % D, i = idx / D;
+    float zk = zk_raw(idx, c);
+    if (c < 3) zk = (zk - comk[c]) + dx[c];
+    const float f = fixed[i];
+    float o = zk * f + z[idx] * (1.f - f);
+    if (noise2) { o = alpha_ts * o + sigma_ts * noise2[idx]; if (c < 3) s2[c] += o; }
+    z[idx] = o;
+  }
+  float com2[3] = {0.f, 0.f, 0.f};
+  if (noise2) {
+    block_sum(s2, 3, red);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) com2[c] = s2[c] / nl;
+    __syncthreads();
+  }
+  for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
+    const size_t r = (size_t)i * D;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float h = (hist[r + c] - comk[c]) + dx[c];
+      if (noise2) { h -= com2[c]; z[r + c] -= com2[c]; }
+      hist[r + c] = h;
+    }
+  }
+  for (int idx = p0 * DR + threadIdx.x; idx < p1 * DR; idx += blockDim.x) {
+    const int c = idx % DR;
+    if (c < 3) {
+      float q = (pocket[idx] - comk[c]) + dx[c];
+      if (noise2) q -= com2[c];
+      pocket[idx] = q;
+    }
+  }
+}
+
+// Joint model: the 2M step of ligand and pocket with the joint COM removal, then ddpm_joint_inpaint_kernel's iteration.  The
+// blend keeps the frame of the unknown part; the jump back's COM removal moves the history with z.
+__device__ __forceinline__ void multistep_repaint_joint(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
+                                                        const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
+                                                        const float* __restrict__ x0_lig, const float* __restrict__ x0_poc,
+                                                        const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
+                                                        const float* __restrict__ nx1, const float* __restrict__ nhl1,
+                                                        const float* __restrict__ nhp1, const float* __restrict__ nx3,
+                                                        const float* __restrict__ nhl3, const float* __restrict__ nhp3,
+                                                        const float* k, const JointSpan& sp, int NL, int A, int R, int commit,
+                                                        float (*red)[4]) {
+  const int D = 3 + A, DR = 3 + R;
+  const float alpha_s = k[5], sigma_s = k[6], alpha_ts = k[7], sigma_ts = k[8];
+  float v[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const float o = multistep_repaint_elem(z_lig, h_lig, eps_lig, (size_t)idx, k, commit);
+    const int c = idx % D;
+    if (c < 3) v[c] += o;
+  }
+  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+    const float o = multistep_repaint_elem(z_poc, h_poc, eps_poc, (size_t)idx, k, commit);
+    const int c = idx % DR;
+    if (c < 3) v[c] += o;
+  }
+  block_sum(v, 3, red);
+  {
+    const float m0 = v[0] / sp.n, m1 = v[1] / sp.n, m2 = v[2] / sp.n;
+    for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
+      const size_t r = (size_t)i * D;
+      z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
+      h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
+    }
+    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
+      const size_t r = (size_t)i * DR;
+      z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
+      h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2;
+    }
+  }
+  __syncthreads();                      // z = the unknown part, complete
+
+  // from here on ddpm_joint_inpaint_kernel, with the history following z through the jump back
+  float n1[3];
+  joint_noise_mean(nx1, sp, NL, red, n1);
+  auto zk_lig = [&](int idx, int c, int i) {
+    const float e = c < 3 ? nx1[(size_t)i * 3 + c] - n1[c] : nhl1[(size_t)i * A + (c - 3)];
+    return alpha_s * x0_lig[idx] + sigma_s * e;
+  };
+  auto zk_poc = [&](int idx, int c, int i) {
+    const float e = c < 3 ? nx1[(size_t)(NL + i) * 3 + c] - n1[c] : nhp1[(size_t)i * R + (c - 3)];
+    return alpha_s * x0_poc[idx] + sigma_s * e;
+  };
+  for (int q = 0; q < 7; ++q) v[q] = 0.f;
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const int c = idx % D, i = idx / D;
+    if (c < 3 && fix_lig[i] != 0.f) { v[c] += z_lig[idx]; v[3 + c] += zk_lig(idx, c, i); if (c == 0) v[6] += 1.f; }
+  }
+  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+    const int c = idx % DR, i = idx / DR;
+    if (c < 3 && fix_poc[i] != 0.f) { v[c] += z_poc[idx]; v[3 + c] += zk_poc(idx, c, i); if (c == 0) v[6] += 1.f; }
+  }
+  block_sum(v, 7, red);
+  const float nf = v[6] > 0.f ? v[6] : 1.f;
+  float shift[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) shift[c] = v[c] / nf - v[3 + c] / nf;
+  float n3[3] = {0.f, 0.f, 0.f};
+  if (nx3) joint_noise_mean(nx3, sp, NL, red, n3);
+  float s[3] = {0.f, 0.f, 0.f};
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const int c = idx % D, i = idx / D;
+    float zk = zk_lig(idx, c, i);
+    if (c < 3) zk += shift[c];
+    const float f = fix_lig[i];
+    float o = zk * f + z_lig[idx] * (1.f - f);
+    if (nx3) {
+      const float e = c < 3 ? nx3[(size_t)i * 3 + c] - n3[c] : nhl3[(size_t)i * A + (c - 3)];
+      o = alpha_ts * o + sigma_ts * e;
+      if (c < 3) s[c] += o;
+    }
+    z_lig[idx] = o;
+  }
+  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+    const int c = idx % DR, i = idx / DR;
+    float zk = zk_poc(idx, c, i);
+    if (c < 3) zk += shift[c];
+    const float f = fix_poc[i];
+    float o = zk * f + z_poc[idx] * (1.f - f);
+    if (nx3) {
+      const float e = c < 3 ? nx3[(size_t)(NL + i) * 3 + c] - n3[c] : nhp3[(size_t)i * R + (c - 3)];
+      o = alpha_ts * o + sigma_ts * e;
+      if (c < 3) s[c] += o;
+    }
+    z_poc[idx] = o;
+  }
+  if (nx3) {
+    block_sum(s, 3, red);
+    const float m0 = s[0] / sp.n, m1 = s[1] / sp.n, m2 = s[2] / sp.n;
+    __syncthreads();
+    for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
+      const size_t r = (size_t)i * D;
+      z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
+      h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
+    }
+    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
+      const size_t r = (size_t)i * DR;
+      z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
+      h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2;
+    }
+  }
+}
+
+// One block per graph; coef row g = the 2M row (5) then the RePaint row (4).
+__global__ void __launch_bounds__(128) ddpm_multistep_inpaint_kernel(
+    float* z_lig, float* z_poc, float* h_lig, float* h_poc, const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
+    const float* __restrict__ known_lig, const float* __restrict__ known_poc, const float* __restrict__ com_pocket0,
+    const float* __restrict__ fix_lig, const float* __restrict__ fix_poc, const float* __restrict__ n1, const float* __restrict__ nhl1,
+    const float* __restrict__ nhp1, const float* __restrict__ n3, const float* __restrict__ nhl3, const float* __restrict__ nhp3,
+    const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP,
+    int A, int R, int joint, int commit) {
+  __shared__ float red[9][4];
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
+  float k[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) k[i] = coef[blockIdx.x * 9 + i];
+  if (joint)
+    multistep_repaint_joint(z_lig, z_poc, h_lig, h_poc, eps_lig, eps_poc, known_lig, known_poc, fix_lig, fix_poc, n1, nhl1, nhp1,
+                            n3, nhl3, nhp3, k, sp, NL, A, R, commit, red);
+  else
+    multistep_repaint_cond(z_lig, z_poc, h_lig, eps_lig, known_lig, com_pocket0, fix_lig, n1, n3, k, sp, A, R, commit, red);
+}
+
 // ---- seeded per-graph random numbers (dsb_seeded_normal; the contract is in include/diffsbdd_b200.h) -------------------
 // Philox4x32-10 (Salmon et al., SC'11): 10 rounds, the key bumped by the Weyl constants between rounds.
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
@@ -1249,6 +1491,31 @@ int dsb_ddpm_multistep_update(float* z_lig, float* z_pocket, float* hist_lig, fl
                                                                              eps_pocket, coef, mask_atoms, mask_residues,
                                                                              (int)n_atoms, (int)n_residues, atom_nf, residue_nf,
                                                                              joint != 0);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
+                                      const float* eps_pocket, const float* known_lig, const float* known_pocket,
+                                      const float* com_pocket0, const float* lig_fixed, const float* pocket_fixed,
+                                      const float* noise_known, const float* noise_known_h_lig, const float* noise_known_h_pocket,
+                                      const float* renoise, const float* renoise_h_lig, const float* renoise_h_pocket,
+                                      const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms,
+                                      int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint,
+                                      int32_t commit, void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!z_lig || !hist_lig || !eps_lig || !known_lig || !lig_fixed || !noise_known || !coef || !mask_atoms ||
+      (n_residues > 0 && (!z_pocket || !mask_residues)) ||
+      (joint ? (!noise_known_h_lig || (renoise && !renoise_h_lig) ||
+                (n_residues > 0 && (!hist_pocket || !eps_pocket || !known_pocket || !pocket_fixed || !noise_known_h_pocket ||
+                                    (renoise && !renoise_h_pocket))))
+             : !com_pocket0)) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  ddpm_multistep_inpaint_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
+      z_lig, z_pocket, hist_lig, hist_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0, lig_fixed, pocket_fixed,
+      noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket, coef, mask_atoms,
+      mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }

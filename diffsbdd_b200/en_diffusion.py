@@ -516,11 +516,15 @@ class EnVariationalDiffusion(nn.Module):
         inp = [self.alpha(gamma_s, s_arr), self.sigma(gamma_s, s_arr), alp_j, sig_j]
         return t_arr.float().contiguous(), torch.cat(rev + inp, dim=1).float().contiguous()
 
-    def _fast_tables(self, timesteps, sampler, eta, device):
+    def _fast_tables(self, timesteps, sampler, eta, device, top=None):
         """Per-step t and coefficients of the 'ddim' / 'dpmpp_2m' steps s = 0..timesteps-1 (t = s+1) for both engines:
-        fast_coefficients in float64 from the fp32 gamma values, cast to fp32, so that eager and graph steps use the same bits."""
+        fast_coefficients in float64 from the fp32 gamma values, cast to fp32, so that eager and graph steps use the same bits.
+        ``top`` = (n, T): the grid ends at t* = n / T instead of 1 (diversify), t_k = k n / (timesteps T) in one rounding."""
         s_int = torch.arange(timesteps, device=device).view(-1, 1)
-        t_arr, s_arr = (s_int + 1) / timesteps, s_int / timesteps
+        if top is None:
+            t_arr, s_arr = (s_int + 1) / timesteps, s_int / timesteps
+        else:
+            t_arr, s_arr = (s_int + 1) * top[0] / (timesteps * top[1]), s_int * top[0] / (timesteps * top[1])
         coef = fast_coefficients(self.gamma(s_arr), self.gamma(t_arr), sampler, eta)
         return t_arr.float().contiguous(), coef.float().contiguous()
 
@@ -552,11 +556,14 @@ class EnVariationalDiffusion(nn.Module):
                           u=torch.zeros(1, dtype=torch.int64, device=device))
             if sampler != 'ddpm':     # few-step samplers: their coefficient table; DDIM at eta = 0 adds 0 * (zeroed noise)
                 _, fast = self._fast_tables(timesteps, sampler, eta, device)
-                st.update(fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device), eta=eta)
+                st.update(fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device), eta=eta,
+                          sampler=sampler)
                 for x in st['n_rev']:
                     x.zero_()
-                if sampler == 'dpmpp_2m':
+                if sampler == 'dpmpp_2m':   # RePaint rounds: the 2M row and the RePaint row in one [n, 9] buffer
                     st['hist'] = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket))
+                    st.update(ms_table=torch.cat((fast, coef_table[:, 3:]), 1).contiguous(),
+                              coef9=torch.zeros((n_samples, 9), device=device))
             self._joint_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -566,11 +573,14 @@ class EnVariationalDiffusion(nn.Module):
     def _joint_step(self, st, kind):
         """kind: 'reverse' (sample: one joint reverse step, step -= 1) | 'inpaint' (noised known part + reverse step + blend,
         step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1) | 'ddim' | 'dpmpp_2m'
-        (_joint_fast_captured_step)."""
+        (_joint_fast_captured_step).  The inpainting kinds of an engine built for a few-step sampler, and its 'inpaint_hold',
+        are _joint_fast_inpaint_captured_step."""
         import ctypes as C
         from . import _native, seeded
         if kind in ('ddim', 'dpmpp_2m'):
             return self._joint_fast_captured_step(st, kind)
+        if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
+            return self._joint_fast_inpaint_captured_step(st, kind)
         dyn, lib = self.dynamics, _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
         NL, NP = st['zl'].shape[0], st['zp'].shape[0]
@@ -737,9 +747,10 @@ class EnVariationalDiffusion(nn.Module):
         dyn.check_status()
         return st['zl'].clone(), st['zp'].clone()
 
-    def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta):
+    def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta, u=0):
         """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s of the joint model (DESIGN §13); ``row`` [1, k]: the step's row of
-        _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step (2M only)."""
+        _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step (2M only).
+        ``u``: the RePaint block of the seeded DDIM draw."""
         from . import seeded
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
@@ -749,7 +760,7 @@ class EnVariationalDiffusion(nn.Module):
             mu_l = zl / cl[:, 0:1] - cl[:, 1:2] * eps_l
             mu_p = zp / cp[:, 0:1] - cp[:, 1:2] * eps_p
             if eta > 0:
-                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
+                self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
                 mu_l, mu_p = self.sample_normal(mu_l, mu_p, c[:, 2:3], lig_mask, pocket_mask)
             zl, zp = self._project_joint_com(mu_l, mu_p, lig_mask, pocket_mask)
             return zl, zp, hl, hp
@@ -762,6 +773,120 @@ class EnVariationalDiffusion(nn.Module):
         for x, m in ((zl, lig_mask), (zp, pocket_mask), (x0_l, lig_mask), (x0_p, pocket_mask)):
             x[:, :nd] -= mean[m]
         return zl, zp, x0_l, x0_p
+
+    def _joint_fast_inpaint_captured_step(self, st, kind):
+        """One RePaint iteration of an engine built for 'ddim' or 'dpmpp_2m' (DESIGN §14).  kind: 'inpaint' (blend; the
+        iteration commits its x0_hat as the 2M history; step -= 1) | 'inpaint_jump' (blend + jump back, no commit; step +=
+        jump_length - 1) | 'inpaint_hold' (blend, no commit, step -= 1: a frame is taken before an eager jump back).  DDIM:
+        native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients -> dsb_ddpm_joint_inpaint_update.  2M: native
+        denoiser -> dsb_ddpm_multistep_inpaint_update."""
+        import ctypes as C
+        from . import _native, seeded
+        dyn, lib = self.dynamics, _native.load()
+        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
+        NL, NP = st['zl'].shape[0], st['zp'].shape[0]
+        ptr = lambda x: x.data_ptr()
+        roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
+        ddim, jump = st['sampler'] == 'ddim', kind == 'inpaint_jump'
+
+        def draw(bufs, purpose):
+            if st['seeded']:
+                for x, role in zip(bufs, roles):
+                    seeded.fill(x, role, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
+            else:
+                for x in bufs:
+                    x.normal_()
+
+        def run():
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            if st['seeded']:
+                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
+            draw(st['n_known'], seeded.PURPOSE_KNOWN)              # eager order: known part, reverse step, jump back
+            idx = st['step'].clamp(min=0)
+            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
+            if ddim:
+                st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
+                st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
+            else:
+                st['coef9'].copy_(st['ms_table'].index_select(0, idx).expand(n, 9))
+            eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
+            if ddim and st['eta'] > 0:
+                draw(st['n_rev'], seeded.PURPOSE_REVERSE)
+            if jump:
+                draw(st['n_jump'], seeded.PURPOSE_RENOISE)
+            kn = st['known']
+            j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
+            if ddim:
+                nx, nhl, nhp = st['n_rev']
+                _native.check(lib.dsb_ddpm_joint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
+                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
+                _native.check(lib.dsb_ddpm_joint_inpaint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
+                    *[ptr(x) for x in st['n_known']], *j, ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n,
+                    self.atom_nf, self.residue_nf, stream))
+            else:
+                hl, hp = st['hist']
+                _native.check(lib.dsb_ddpm_multistep_inpaint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(kn['xl']), ptr(kn['xp']), None,
+                    ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st['coef9']), ptr(lm), ptr(pm),
+                    NL, NP, n, self.atom_nf, self.residue_nf, 1, int(kind == 'inpaint'), stream))
+            if jump:
+                st['step'].add_(st['jump'] - 1)
+                if st['seeded']:
+                    st['u'].add_(1)
+            else:
+                st['step'].sub_(1)
+        return run
+
+    def _joint_fast_inpaint_step(self, s, i, t, row, gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket, lig_fixed,
+                                 pocket_fixed, lsel, psel, lmask, pmask, sampler, eta, commit):
+        """Eager RePaint iteration (s, block i) of the joint inpaint with the 'ddim' / 'dpmpp_2m' step (DESIGN §14), without
+        the jump back (_joint_renoise).  ``hist``: () for DDIM; for 2M (hist_lig, hist_pocket) = x0_hat committed by the last
+        iteration of step s + 1, in the frame of z.  The 2M COM removal moves it with z; the blend keeps the frame of the
+        unknown part, so nothing else moves it; ``commit``: this iteration's x0_hat becomes the history.  Returns
+        (z_lig, z_pocket, hist)."""
+        from . import seeded
+        nd = self.n_dims
+        self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_KNOWN)
+        zk_lig, zk_pocket, _, _ = self.noised_representation(xh0_lig, xh0_pocket, lmask, pmask, gamma_s)
+        if sampler == 'ddim':
+            zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, None, None, lmask, pmask, sampler, eta, i)
+        else:
+            c = row.expand(t.shape[0], -1)
+            cl, cp = c[lmask], c[pmask]
+            hl, hp = (x.clone() for x in hist)
+            eps_l, eps_p = self.dynamics(z_lig, z_pocket, t, lmask, pmask)
+            x0_l = (z_lig - cl[:, 3:4] * eps_l) * cl[:, 2:3]
+            x0_p = (z_pocket - cp[:, 3:4] * eps_p) * cp[:, 2:3]
+            zu_lig = cl[:, 0:1] * z_lig + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0_l - cl[:, 4:5] * hl)
+            zu_pocket = cp[:, 0:1] * z_pocket + cp[:, 1:2] * ((1 + cp[:, 4:5]) * x0_p - cp[:, 4:5] * hp)
+            mean = scatter_mean(torch.cat((zu_lig[:, :nd], zu_pocket[:, :nd])), torch.cat((lmask, pmask)), dim=0,
+                                dim_size=t.shape[0])
+            for x, m in ((zu_lig, lmask), (zu_pocket, pmask), (x0_l, lmask), (x0_p, pmask), (hl, lmask), (hp, pmask)):
+                x[:, :nd] -= mean[m]
+            hist = (x0_l, x0_p) if commit else (hl, hp)
+        # the rest is _inpaint's iteration
+        shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
+            self._fixed_com(zk_lig[:, :nd], zk_pocket[:, :nd], lsel, psel, lmask, pmask)
+        zk_lig[:, :nd] = zk_lig[:, :nd] + shift[lmask]
+        zk_pocket[:, :nd] = zk_pocket[:, :nd] + shift[pmask]
+        z_lig = zk_lig * lig_fixed + zu_lig * (1 - lig_fixed)
+        z_pocket = zk_pocket * pocket_fixed + zu_pocket * (1 - pocket_fixed)
+        return z_lig, z_pocket, hist
+
+    def _joint_renoise(self, z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask):
+        """sample_p_zt_given_zs (the jump back) with the 2M history ``hist`` (or ()) moved by the same joint COM removal."""
+        nd = self.n_dims
+        _, sigma_ts, alpha_ts = self.sigma_and_alpha_t_given_s(gamma_t, gamma_s, z_lig)
+        zl, zp = self.sample_normal(alpha_ts[lmask] * z_lig, alpha_ts[pmask] * z_pocket, sigma_ts, lmask, pmask)
+        mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lmask, pmask)), dim=0)
+        moved = []
+        for x, m in ((zl, lmask), (zp, pmask)) + tuple(zip(hist, (lmask, pmask))):
+            x = x.clone()
+            x[:, :nd] = x[:, :nd] - mean[m]
+            moved.append(x)
+        return moved[0], moved[1], tuple(moved[2:])
 
     @follows_dynamics_determinism
     @torch.no_grad()
@@ -869,14 +994,23 @@ class EnVariationalDiffusion(nn.Module):
     @follows_dynamics_determinism
     @torch.no_grad()
     def inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings=1, jump_length=1, return_frames=1,
-                timesteps=None, seeds=None):
-        """en_diffusion.py:677-837: sample the free nodes while the fixed ones follow q(z_s | x).  ``seeds``: as sample."""
+                timesteps=None, seeds=None, sampler='ddpm', eta=0.0):
+        """en_diffusion.py:677-837: sample the free nodes while the fixed ones follow q(z_s | x).  ``seeds``: as sample.
+        ``sampler`` / ``eta``: the reverse step of every RePaint iteration, as sample; 'dpmpp_2m' needs jump_length = 1
+        (DESIGN §14).  With every pocket node fixed this is how a joint model generates a ligand for a given pocket in few
+        steps."""
         from . import seeded
+        check_sampler(sampler, eta)
+        if sampler == 'dpmpp_2m' and jump_length > 1:
+            raise ValueError(f"sampler='dpmpp_2m' needs jump_length = 1 (got {jump_length}): its history has no rule for "
+                             f"jumps over several steps; use 'ddim'")
         seeds = seeded.as_seeds(seeds, len(ligand['size']), ligand['x'].device)
         with self._seeded(seeds, ligand['mask'], pocket['mask']):
-            return self._inpaint(ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps)
+            return self._inpaint(ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps,
+                                 sampler, float(eta))
 
-    def _inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps):
+    def _inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings, jump_length, return_frames, timesteps,
+                 sampler='ddpm', eta=0.0):
         from . import seeded
         timesteps = self.T if timesteps is None else timesteps
         if self._rng is not None:          # u counts the jump-back blocks of the RePaint schedule
@@ -911,7 +1045,8 @@ class EnVariationalDiffusion(nn.Module):
         s = timesteps - 1
         if self._joint_use_graph(z_lig.device):
             dyn = self.dynamics
-            st = self._joint_engine(z_lig, z_pocket, lmask, pmask, n_samples, timesteps, jump_length)
+            st = self._joint_engine(z_lig, z_pocket, lmask, pmask, n_samples, timesteps, jump_length, sampler, eta)
+            two_m = sampler == 'dpmpp_2m'
             if st['known'] is None:       # static buffers the captured RePaint iteration reads
                 st['known'] = dict(xl=torch.empty_like(xh0_lig), xp=torch.empty_like(xh0_pocket),
                                    fl=torch.empty(len(lmask), device=z_lig.device), fp=torch.empty(len(pmask), device=z_lig.device))
@@ -921,14 +1056,21 @@ class EnVariationalDiffusion(nn.Module):
             try:
                 g_it = self._joint_graph(st, 'inpaint', z_lig, z_pocket, s)
                 g_jump = self._joint_graph(st, 'inpaint_jump', z_lig, z_pocket, s) if len(schedule) > 1 else None
+                # 2M: the frame-before-jump path replays an iteration that does not commit (captured here: a capture
+                # resets the static state)
+                g_hold = self._joint_graph(st, 'inpaint_hold', z_lig, z_pocket, s) if two_m and len(schedule) > 1 else None
                 self._joint_start(st, z_lig, z_pocket, s)
                 for i, n_denoise in enumerate(schedule):
                     for j in range(n_denoise):
                         jump = j == n_denoise - 1 and i < len(schedule) - 1
                         frame = (n_denoise > jump_length or i == len(schedule) - 1) and (s * return_frames) % timesteps == 0
                         # a frame is taken after the blend and BEFORE the jump back (en_diffusion.py:777-788): in that case the
-                        # jump runs as eager torch ops on the static state instead of inside the fused kernel
-                        (g_jump if (jump and not frame) else g_it).replay()
+                        # jump runs as eager torch ops on the static state instead of inside the fused kernel (2M: after an
+                        # iteration that does not commit)
+                        if jump and frame and two_m:
+                            g_hold.replay()
+                        else:
+                            (g_jump if (jump and not frame) else g_it).replay()
                         if frame:
                             idx = (s * return_frames) // timesteps
                             out_lig[idx], out_pocket[idx] = self.unnormalize_z(st['zl'], st['zp'])
@@ -937,9 +1079,14 @@ class EnVariationalDiffusion(nn.Module):
                                 self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
                                 s_arr = torch.full((n_samples, 1), fill_value=s, device=z_lig.device) / timesteps
                                 t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
-                                zl, zp = self.sample_p_zt_given_zs(
-                                    st['zl'], st['zp'], lmask, pmask, self.inflate_batch_array(self.gamma(t_back), ligand['x']),
-                                    self.inflate_batch_array(self.gamma(s_arr), ligand['x']))
+                                g_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
+                                g_s = self.inflate_batch_array(self.gamma(s_arr), ligand['x'])
+                                if two_m:
+                                    zl, zp, hist = self._joint_renoise(st['zl'], st['zp'], st['hist'], g_t, g_s, lmask, pmask)
+                                    for x, y in zip(st['hist'], hist):
+                                        x.copy_(y)
+                                else:
+                                    zl, zp = self.sample_p_zt_given_zs(st['zl'], st['zp'], lmask, pmask, g_t, g_s)
                                 st['zl'].copy_(zl); st['zp'].copy_(zp); st['step'].add_(jump_length)
                                 if st['seeded']:
                                     st['u'].add_(1)
@@ -950,6 +1097,28 @@ class EnVariationalDiffusion(nn.Module):
             dyn.check_status()
             z_lig, z_pocket = st['zl'].clone(), st['zp'].clone()
             self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :nd], z_pocket[:, :nd]), dim=0), combined_mask)
+        elif sampler != 'ddpm':
+            t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
+            hist = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket)) if sampler == 'dpmpp_2m' else ()
+            for i, n_denoise in enumerate(schedule):
+                for j in range(n_denoise):
+                    jump = j == n_denoise - 1 and i < len(schedule) - 1
+                    s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device) / timesteps
+                    gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
+                    z_lig, z_pocket, hist = self._joint_fast_inpaint_step(
+                        s, i, t_table[s].expand(n_samples, 1), coef[s:s + 1], gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket,
+                        lig_fixed, pocket_fixed, lsel, psel, lmask, pmask, sampler, eta, not jump)
+                    self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :nd], z_pocket[:, :nd]), dim=0), combined_mask)
+                    if (n_denoise > jump_length or i == len(schedule) - 1) and (s * return_frames) % timesteps == 0:
+                        idx = (s * return_frames) // timesteps
+                        out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
+                    if jump:                                           # jump back jump_length steps
+                        t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
+                        gamma_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
+                        self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
+                        z_lig, z_pocket, hist = self._joint_renoise(z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask)
+                        s = s + jump_length
+                    s -= 1
         else:
             for i, n_denoise in enumerate(schedule):
                 for j in range(n_denoise):

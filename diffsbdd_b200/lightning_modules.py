@@ -177,12 +177,13 @@ class LigandPocketDDPM(_Base):
         (lightning_modules.py:785-852): returns (xh_lig, xh_pocket, lig_mask, pocket_mask) in the original
         pocket frame.  ``seeds``: one int64 per sample (seeded.py); the ligand size prior and every sampler draw then come
         from the sample's own seed (the size by inverse CDF over p(n_lig | n_pocket)).  ``sampler`` / ``eta``: the reverse
-        step of ConditionalDDPM.sample_given_pocket; a joint model generates through RePaint inpainting, which has only
-        the 'ddpm' step."""
+        step of ConditionalDDPM.sample_given_pocket.  A joint model refuses a few-step sampler here: this route runs its
+        RePaint inpainting with the 'ddpm' step.  Few-step generation for a fixed pocket with a joint model is
+        ``self.ddpm.inpaint(ligand, pocket, lig_fixed=zeros, pocket_fixed=ones, sampler=..., eta=...)`` (DESIGN §14)."""
         check_sampler(sampler, eta)
         if sampler != 'ddpm' and type(self.ddpm) == EnVariationalDiffusion:
             raise ValueError(f"sampler={sampler!r} is not supported for a joint model: it generates through RePaint inpainting, "
-                             f"which runs the 'ddpm' step only")
+                             f"which runs the 'ddpm' step only here (use ddpm.inpaint with every pocket node fixed and sampler=...)")
         self.ddpm.eval()
         seeds = seeded.as_seeds(seeds, len(pocket['size']), pocket['x'].device)
         pocket_com_before = scatter_mean(pocket['x'], pocket['mask'], dim=0)

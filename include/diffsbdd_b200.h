@@ -277,6 +277,36 @@ int dsb_ddpm_multistep_update(float* z_lig, float* z_pocket, float* hist_lig, fl
                               const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
                               int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream);
 
+/* ---- RePaint round with the DPM-Solver++(2M) step (one launch, one block per graph; DESIGN §14), both models.  On entry z is
+ * z_t of the round; per graph, in place:
+ *   1. the 2M step of dsb_ddpm_multistep_update: x0 = (z - sigma_t eps_hat) * inv_alpha_t ; D = (1 + w) x0 - w hist (x0 when
+ *      w == 0) ; z' = c0 z + c1 D ; the COM of z'.x removed (joint == 0: ligand COM from z', the pocket and hist ;
+ *      joint != 0: ligand + pocket COM from z' and hist of both).
+ *   2. the RePaint iteration on z' as the unknown part:
+ *      joint == 0: dsb_ddpm_inpaint_update with (known_lig, com_pocket0, lig_fixed, noise_known, renoise); known_pocket,
+ *                  pocket_fixed, eps_pocket, hist_pocket and the *_h_* noises are not used and may be NULL.
+ *      joint != 0: dsb_ddpm_joint_inpaint_update with (known_lig, known_pocket, lig_fixed, pocket_fixed, noise_known +
+ *                  noise_known_h_*, renoise + renoise_h_*); com_pocket0 is not used and may be NULL.
+ *      renoise == NULL: no re-noising (the round that ends a grid step).
+ * hist_* [rows, 3 + nf]: x0 of the previous grid step, in the frame of the pocket (joint == 0) or of z (joint != 0).  Every
+ * translation the round applies to the pocket coordinates (joint == 0: the 2M COM removal, the known part's COM removal, the
+ * fixed-COM shift, the re-noise COM removal) or to z (joint != 0: the 2M and the re-noise COM removals) is applied to hist.x as
+ * well.  commit != 0: x0 of this round replaces the history before those translations; commit == 0: the history is only
+ * translated.
+ * coef: device fp32 [n_graphs, 9] = (sigma_s/sigma_t, -alpha_s (e^-h - 1), 1/alpha_t, sigma_t, w) as dsb_ddpm_multistep_update,
+ * then (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}) as the RePaint entries.  Noise layouts as dsb_ddpm_inpaint_update
+ * (joint == 0: [n_atoms, 3 + atom_nf]) and dsb_ddpm_joint_inpaint_update (joint != 0: x [n_atoms + n_residues, 3], h per part).
+ * Masks sorted; each graph's sums run in a fixed order without atomics, so the result repeats bit for bit and a graph's result
+ * does not depend on the rest of its batch. */
+int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
+                                      const float* eps_pocket, const float* known_lig, const float* known_pocket,
+                                      const float* com_pocket0, const float* lig_fixed, const float* pocket_fixed,
+                                      const float* noise_known, const float* noise_known_h_lig, const float* noise_known_h_pocket,
+                                      const float* renoise, const float* renoise_h_lig, const float* renoise_h_pocket,
+                                      const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms,
+                                      int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint,
+                                      int32_t commit, void* stream);
+
 /* ---- evaluation-mode variational bound (validation / test NLL): what EnVariationalDiffusion.forward, ConditionalDDPM.forward
  * and SimpleConditionalDDPM.forward compute in eval mode besides the two denoiser calls and the per-graph scalar algebra.
  *
