@@ -450,15 +450,20 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
     def _fast_inpaint_step(self, s, u, t, row, gamma_s, gamma_t, z_lig, xh_pocket, hist, ligand_x, xh_ligand, com_pocket_0,
                            lig_fixed, lmask, pmask, sampler, eta, last):
-        """Eager RePaint round (s, u) with the 'ddim' / 'dpmpp_2m' step (DESIGN §14): _inpaint's iteration with the few-step
-        step in place of the ancestral one; ``row`` [1, k]: the step's row of _fast_tables, ``last``: no re-noising after
-        this round.  2M: ``hist`` is x0_hat committed by the last round of step s + 1, kept in the pocket's frame: every
-        translation of the pocket coordinates moves it too, and the last round of step s commits its own x0_hat.  Returns
-        (z_lig, xh_pocket, hist)."""
+        """Eager RePaint round (s, u) of _inpaint (DESIGN §14): the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row``
+        and t; 'ddim' / 'dpmpp_2m': the few-step step with ``row`` [1, k], the step's row of _fast_tables), then the known
+        part, the COM alignment, the blend and, unless ``last``, the re-noising.  2M: ``hist`` is x0_hat committed by the
+        last round of step s + 1, kept in the pocket's frame: every translation of the pocket coordinates moves it too, and
+        the last round of step s commits its own x0_hat.  Returns (z_lig, xh_pocket, hist)."""
         nd, NL, NP = self.n_dims, z_lig.shape[0], xh_pocket.shape[0]
         fixed_rows = lig_fixed.bool().view(-1)
-        if sampler == 'ddim':
+        if sampler == 'ddpm':
+            self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
+            z_unknown, xh_pocket = self.sample_p_zs_given_zt(row, t, z_lig, xh_pocket, lmask, pmask)
+        elif sampler == 'ddim':
             z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u)
+        if sampler != 'dpmpp_2m':
+            # only the x columns of the pocket are ever translated
             frame, fmask = xh_pocket[:, :nd], pmask
         else:
             c = row.expand(t.shape[0], -1)[lmask]
@@ -470,11 +475,12 @@ class ConditionalDDPM(EnVariationalDiffusion):
             z_unknown[:, :nd], frame = self.remove_mean_batch(
                 z_unknown[:, :nd], torch.cat((xh_pocket[:, :nd], hist[:, :nd], x0[:, :nd])), lmask, fmask)
 
-        # the rest is _inpaint's iteration, with ``frame`` in place of the pocket coordinates
+        # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
         com_pocket = scatter_mean(frame[:NP], pmask, dim=0)
         xh_ligand[:, :nd] = ligand_x + (com_pocket - com_pocket_0)[lmask]
         self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_KNOWN)
         z_known, frame, _ = self.noised_representation(xh_ligand, frame, lmask, fmask, gamma_s)
+        # align COM of the fixed atoms: noised -> denoised (conditional_model.py:645-656)
         com_noised = scatter_mean(z_known[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
         com_denoised = scatter_mean(z_unknown[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
         dx = com_denoised - com_noised
@@ -651,15 +657,13 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + xh_pocket.size(), device=device)
-        use_graph = self._use_graph(device)
-        nd = self.n_dims
-
-        if use_graph:
+        if self._use_graph(device):
             z_lig, xh_pocket = self._graphed_inpaint_loop(z_lig, xh_pocket, xh_ligand, com_pocket_0, lig_fixed, lmask, pmask,
                                                          n_samples, timesteps, resamplings, return_frames, out_lig, out_pocket,
                                                          sampler, eta)
-        elif sampler != 'ddpm':
-            t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
+        else:
+            if sampler != 'ddpm':
+                t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
             hist = torch.zeros_like(z_lig)
             for s in reversed(range(0, timesteps)):
                 for u in range(resamplings):
@@ -667,42 +671,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
                     t_array = (s_array + 1) / timesteps
                     s_array = s_array / timesteps
                     last = u == resamplings - 1
+                    t, row = (t_array, s_array) if sampler == 'ddpm' else (t_table[s].expand(n_samples, 1), coef[s:s + 1])
                     z_lig, xh_pocket, hist = self._fast_inpaint_step(
-                        s, u, t_table[s].expand(n_samples, 1), coef[s:s + 1], self.gamma(s_array), self.gamma(t_array), z_lig,
-                        xh_pocket, hist, ligand['x'], xh_ligand, com_pocket_0, lig_fixed, lmask, pmask, sampler, eta, last)
+                        s, u, t, row, self.gamma(s_array), self.gamma(t_array), z_lig, xh_pocket, hist, ligand['x'], xh_ligand,
+                        com_pocket_0, lig_fixed, lmask, pmask, sampler, eta, last)
                     if last and (s * return_frames) % timesteps == 0:
-                        idx = (s * return_frames) // timesteps
-                        out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
-        else:
-            for s in reversed(range(0, timesteps)):
-                for u in range(resamplings):
-                    s_array = torch.full((n_samples, 1), fill_value=s, device=device)
-                    t_array = (s_array + 1) / timesteps
-                    s_array = s_array / timesteps
-                    gamma_t, gamma_s = self.gamma(t_array), self.gamma(s_array)
-
-                    # denoise the whole ligand one step (unknown part)
-                    self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
-                    z_unknown, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, xh_pocket, lmask, pmask)
-
-                    # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
-                    com_pocket = scatter_mean(xh_pocket[:, :nd], pmask, dim=0)
-                    xh_ligand[:, :nd] = ligand['x'] + (com_pocket - com_pocket_0)[lmask]
-                    self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_KNOWN)
-                    z_known, xh_pocket, _ = self.noised_representation(xh_ligand, xh_pocket, lmask, pmask, gamma_s)
-
-                    # align COM of the fixed atoms: noised -> denoised (conditional_model.py:645-656)
-                    com_noised = scatter_mean(z_known[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
-                    com_denoised = scatter_mean(z_unknown[fixed_rows][:, :nd], lmask[fixed_rows], dim=0)
-                    dx = com_denoised - com_noised
-                    z_known[:, :nd] = z_known[:, :nd] + dx[lmask]
-                    xh_pocket[:, :nd] = xh_pocket[:, :nd] + dx[pmask]
-
-                    z_lig = z_known * lig_fixed + z_unknown * (1 - lig_fixed)
-                    if u < resamplings - 1:
-                        self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_RENOISE)
-                        z_lig, xh_pocket = self.sample_p_zt_given_zs(z_lig, xh_pocket, lmask, pmask, gamma_t, gamma_s)
-                    if u == resamplings - 1 and (s * return_frames) % timesteps == 0:
                         idx = (s * return_frames) // timesteps
                         out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
 

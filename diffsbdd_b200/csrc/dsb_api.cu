@@ -357,11 +357,31 @@ static int check_sizes(int64_t NL, int64_t NP, int64_t B, int64_t Ecap) {
   return 0;
 }
 
-// ---- fused DDPM ligand update --------------------------------------------------------------------------
+// ---- fused DDPM updates: per-graph spans and translations ----------------------------------------------------------------
 __device__ __forceinline__ int lb64(const int64_t* a, int n, int64_t v) {
   int lo = 0, hi = n;
   while (lo < hi) { int mid = (lo + hi) >> 1; if (a[mid] < v) lo = mid + 1; else hi = mid; }
   return lo;
+}
+
+// Graph g: ligand rows [l0, l1) of the ligand tensors, pocket rows [p0, p1) of the pocket tensors; n = its ligand + pocket
+// node count (1 for an empty graph).
+struct JointSpan { int l0, l1, p0, p1; float n; };
+__device__ __forceinline__ JointSpan joint_span(const int64_t* mask_atoms, const int64_t* mask_res, int NL, int NP, int g) {
+  JointSpan s;
+  s.l0 = lb64(mask_atoms, NL, g); s.l1 = lb64(mask_atoms, NL, (int64_t)g + 1);
+  s.p0 = lb64(mask_res, NP, g); s.p1 = lb64(mask_res, NP, (int64_t)g + 1);
+  const int cnt = (s.l1 - s.l0) + (s.p1 - s.p0);
+  s.n = cnt > 0 ? (float)cnt : 1.f;
+  return s;
+}
+
+// x[i * stride + c] -= m[c] for the coordinate columns c < 3 of rows i in [r0, r1): one translation of a graph's nodes.
+__device__ __forceinline__ void sub_rows3(float* x, int r0, int r1, int stride, const float* m) {
+  for (int i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
+    const size_t r = (size_t)i * stride;
+    x[r] -= m[0]; x[r + 1] -= m[1]; x[r + 2] -= m[2];
+  }
 }
 
 // z/z_out and pocket/pocket_out may alias (in-place use is part of the contract): no __restrict__ on those pairs.
@@ -371,12 +391,11 @@ __global__ void __launch_bounds__(128) ddpm_update_kernel(const float* z, const 
                                                            const float* pocket, int NL, int NP, int A, int R,
                                                            float* z_out, float* pocket_out) {
   const int g = blockIdx.x;
-  const int l0 = lb64(mask_atoms, NL, g), l1 = lb64(mask_atoms, NL, (int64_t)g + 1);
-  const int p0 = lb64(mask_res, NP, g), p1 = lb64(mask_res, NP, (int64_t)g + 1);
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
   const int D = 3 + A, DR = 3 + R;
   const float alpha = coef[g * 3 + 0], cb = coef[g * 3 + 1], sigma = coef[g * 3 + 2];
   float s[3] = {0.f, 0.f, 0.f};
-  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
     const float mu = z[idx] / alpha - cb * eps[idx];          // conditional_model.py:451-453
     const float v = mu + sigma * noise[idx];                   // conditional_model.py:151
     z_out[idx] = v;
@@ -391,15 +410,13 @@ __global__ void __launch_bounds__(128) ddpm_update_kernel(const float* z, const 
     for (int o = 16; o > 0; o >>= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
   if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = s[0]; red[1][threadIdx.x >> 5] = s[1]; red[2][threadIdx.x >> 5] = s[2]; }
   __syncthreads();
-  if (threadIdx.x < 3) {
-    const float cnt = (l1 - l0) > 0 ? (float)(l1 - l0) : 1.f;
+  if (threadIdx.x < 3) {    // ((r0 + r1) + r2) + r3: not block_sum's order, which would change the sampler's bits
+    const float cnt = (sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f;
     com[threadIdx.x] = (red[threadIdx.x][0] + red[threadIdx.x][1] + red[threadIdx.x][2] + red[threadIdx.x][3]) / cnt;
   }
   __syncthreads();
-  for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {     // conditional_model.py:694
-    z_out[(size_t)i * D + 0] -= com[0]; z_out[(size_t)i * D + 1] -= com[1]; z_out[(size_t)i * D + 2] -= com[2];
-  }
-  for (int idx = p0 * DR + threadIdx.x; idx < p1 * DR; idx += blockDim.x) {   // conditional_model.py:695
+  sub_rows3(z_out, sp.l0, sp.l1, D, com);                       // conditional_model.py:694
+  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {   // conditional_model.py:695
     const int c = idx % DR;
     const float v = pocket[idx];
     pocket_out[idx] = c < 3 ? v - com[c] : v;
@@ -407,7 +424,6 @@ __global__ void __launch_bounds__(128) ddpm_update_kernel(const float* z, const 
 }
 
 
-// ---- fused RePaint iteration of ConditionalDDPM.inpaint (conditional_model.py:636-666) -------------------------------
 // sum of `nv` (<= 9) per-thread values over a 128-thread block; result valid in every thread.  `red` is [9][4] shared floats.
 __device__ __forceinline__ void block_sum(float* v, int nv, float (*red)[4]) {
   for (int k = 0; k < nv; ++k)
@@ -419,23 +435,21 @@ __device__ __forceinline__ void block_sum(float* v, int nv, float (*red)[4]) {
   for (int k = 0; k < nv; ++k) v[k] = (red[k][0] + red[k][1]) + (red[k][2] + red[k][3]);
 }
 
-// One block per graph.  On entry z = z_unknown (the reverse step's output), pocket = the pocket that step left.  In place:
+// ---- RePaint iteration of ConditionalDDPM.inpaint (conditional_model.py:636-666; eager: _fast_inpaint_step) ------------
+// One block per graph, in place.  On entry z = z_unknown (the reverse step's output), pocket = the pocket that step left:
 //   known part noised to level s around the pocket's current COM, ligand-COM removed (noised_representation, :162-183),
-//   COM of the fixed atoms aligned noised -> denoised (:645-656), blend (:659), optional re-noising step
+//   COM of the fixed atoms aligned noised -> denoised (:645-656), blend (:659), and with noise2 the re-noising step
 //   z_t ~ q(z_t | z_s) with its own COM removal (sample_p_zt_given_zs, :420-430, :662-666).
-// Every per-element fp32 operation is the one the torch ops of the eager loop perform, in the same order; only the
-// per-graph means are summed in a different order.
-__global__ void __launch_bounds__(128) ddpm_inpaint_kernel(float* z, float* pocket, const float* __restrict__ known,
-                                                            const float* __restrict__ com_pocket0, const float* __restrict__ fixed,
-                                                            const float* __restrict__ noise1, const float* __restrict__ noise2,
-                                                            const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms,
-                                                            const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R) {
-  const int g = blockIdx.x;
-  const int l0 = lb64(mask_atoms, NL, g), l1 = lb64(mask_atoms, NL, (int64_t)g + 1);
-  const int p0 = lb64(mask_res, NP, g), p1 = lb64(mask_res, NP, (int64_t)g + 1);
+// coef = (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}).  hist (the 2M history, or null) takes every translation of the pocket
+// coordinates, so that it stays in the pocket's frame.  Every per-element fp32 operation is the one the torch ops of the
+// eager loop perform, in the same order; only the per-graph means are summed in a different order.
+__device__ __forceinline__ void repaint_cond(float* z, float* pocket, float* hist, const float* __restrict__ known,
+                                             const float* __restrict__ com_pocket0, const float* __restrict__ fixed,
+                                             const float* __restrict__ noise1, const float* __restrict__ noise2,
+                                             const float* coef, const JointSpan& sp, int A, int R, float (*red)[4]) {
+  const int g = blockIdx.x, l0 = sp.l0, l1 = sp.l1, p0 = sp.p0, p1 = sp.p1;
   const int D = 3 + A, DR = 3 + R;
-  const float alpha_s = coef[g * 4 + 0], sigma_s = coef[g * 4 + 1], alpha_ts = coef[g * 4 + 2], sigma_ts = coef[g * 4 + 3];
-  __shared__ float red[9][4];
+  const float alpha_s = coef[0], sigma_s = coef[1], alpha_ts = coef[2], sigma_ts = coef[3];
   const float nl = (l1 - l0) > 0 ? (float)(l1 - l0) : 1.f, np_ = (p1 - p0) > 0 ? (float)(p1 - p0) : 1.f;
 
   // pocket COM now vs. at the start: the known ligand follows the pocket (:636-640)
@@ -489,8 +503,18 @@ __global__ void __launch_bounds__(128) ddpm_inpaint_kernel(float* z, float* pock
 #pragma unroll
     for (int c = 0; c < 3; ++c) com2[c] = s2[c] / nl;
     __syncthreads();
+    sub_rows3(z, l0, l1, D, com2);
+  }
+  // the pocket coordinates (and the history with them) move by -comk + dx, then by -com2
+  if (hist) {
     for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
-      z[(size_t)i * D + 0] -= com2[0]; z[(size_t)i * D + 1] -= com2[1]; z[(size_t)i * D + 2] -= com2[2];
+      const size_t r = (size_t)i * D;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        float h = (hist[r + c] - comk[c]) + dx[c];
+        if (noise2) h -= com2[c];
+        hist[r + c] = h;
+      }
     }
   }
   for (int idx = p0 * DR + threadIdx.x; idx < p1 * DR; idx += blockDim.x) {
@@ -503,20 +527,21 @@ __global__ void __launch_bounds__(128) ddpm_inpaint_kernel(float* z, float* pock
   }
 }
 
+// dsb_ddpm_inpaint_update: the conditional RePaint iteration after the reverse step.
+__global__ void __launch_bounds__(128) ddpm_inpaint_kernel(float* z, float* pocket, const float* __restrict__ known,
+                                                            const float* __restrict__ com_pocket0, const float* __restrict__ fixed,
+                                                            const float* __restrict__ noise1, const float* __restrict__ noise2,
+                                                            const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms,
+                                                            const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R) {
+  __shared__ float red[9][4];
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
+  repaint_cond(z, pocket, nullptr, known, com_pocket0, fixed, noise1, noise2, coef + blockIdx.x * 4, sp, A, R, red);
+}
+
 
 // ---- joint model (EnVariationalDiffusion): fused reverse update and fused RePaint iteration ---------------------------
-// Node n of graph g: ligand rows [l0, l1) of the ligand tensors, pocket rows [p0, p1) of the pocket tensors.  The position
-// noise nx is ONE tensor [NL + NP, 3] (ligand rows first), as sample_center_gravity_zero_gaussian_batch draws it
-// (en_diffusion.py:559-578); its per-graph mean over ligand+pocket nodes is removed before use (en_diffusion.py:940-944).
-struct JointSpan { int l0, l1, p0, p1; float n; };
-__device__ __forceinline__ JointSpan joint_span(const int64_t* mask_atoms, const int64_t* mask_res, int NL, int NP, int g) {
-  JointSpan s;
-  s.l0 = lb64(mask_atoms, NL, g); s.l1 = lb64(mask_atoms, NL, (int64_t)g + 1);
-  s.p0 = lb64(mask_res, NP, g); s.p1 = lb64(mask_res, NP, (int64_t)g + 1);
-  const int cnt = (s.l1 - s.l0) + (s.p1 - s.p0);
-  s.n = cnt > 0 ? (float)cnt : 1.f;
-  return s;
-}
+// The position noise nx is ONE tensor [NL + NP, 3] (ligand rows first), as sample_center_gravity_zero_gaussian_batch draws
+// it (en_diffusion.py:559-578); its per-graph mean over ligand+pocket nodes is removed before use (en_diffusion.py:940-944).
 // per-graph mean of the position noise rows
 __device__ __forceinline__ void joint_noise_mean(const float* nx, const JointSpan& sp, int NL, float (*red)[4], float* mean) {
   float v[3] = {0.f, 0.f, 0.f};
@@ -558,32 +583,29 @@ __global__ void __launch_bounds__(128) ddpm_joint_update_kernel(float* z_lig, fl
     if (c < 3) s[c] += v;
   }
   block_sum(s, 3, red);
-  const float m0 = s[0] / sp.n, m1 = s[1] / sp.n, m2 = s[2] / sp.n;
+  const float m[3] = {s[0] / sp.n, s[1] / sp.n, s[2] / sp.n};
   __syncthreads();
-  for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
-    z_lig[(size_t)i * D] -= m0; z_lig[(size_t)i * D + 1] -= m1; z_lig[(size_t)i * D + 2] -= m2;
-  }
-  for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
-    z_poc[(size_t)i * DR] -= m0; z_poc[(size_t)i * DR + 1] -= m1; z_poc[(size_t)i * DR + 2] -= m2;
-  }
+  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
 }
 
-// One RePaint iteration of EnVariationalDiffusion.inpaint after the reverse step (en_diffusion.py:741-807), in place on
-// (z_lig, z_poc) = the denoised "unknown" sample:
+// ---- RePaint iteration of EnVariationalDiffusion.inpaint (en_diffusion.py:741-807; eager: _joint_fast_inpaint_step and
+// _joint_renoise).  One block per graph, in place on (z_lig, z_poc) = the denoised "unknown" sample:
 //   z_known = alpha_s xh0 + sigma_s eps1 (eps1.x COM-free)                                  (noised_representation, :302-317)
 //   shift   = COM_fixed(z_unknown) - COM_fixed(z_known) over the fixed ligand+pocket nodes ; z_known.x += shift   (:751-772)
 //   z       = z_known * fixed + z_unknown * (1 - fixed)                                       (:774-775)
 //   if nx3: z = alpha_ts z + sigma_ts eps3 (eps3.x COM-free), joint COM of z.x removed        (sample_p_zt_given_zs, :479-501, :790-807)
-__global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
-    float* z_lig, float* z_poc, const float* __restrict__ x0_lig, const float* __restrict__ x0_poc, const float* __restrict__ fix_lig,
-    const float* __restrict__ fix_poc, const float* __restrict__ nx1, const float* __restrict__ nhl1, const float* __restrict__ nhp1,
-    const float* __restrict__ nx3, const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* __restrict__ coef,
-    const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R) {
-  const int g = blockIdx.x;
-  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
+// coef = (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}).  The blend keeps the frame of the unknown part; the 2M history (h_lig,
+// h_poc, or null) moves with z through the jump back's COM removal.
+__device__ __forceinline__ void repaint_joint(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
+                                              const float* __restrict__ x0_lig, const float* __restrict__ x0_poc,
+                                              const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
+                                              const float* __restrict__ nx1, const float* __restrict__ nhl1,
+                                              const float* __restrict__ nhp1, const float* __restrict__ nx3,
+                                              const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* coef,
+                                              const JointSpan& sp, int NL, int A, int R, float (*red)[4]) {
   const int D = 3 + A, DR = 3 + R;
-  const float alpha_s = coef[g * 4 + 0], sigma_s = coef[g * 4 + 1], alpha_ts = coef[g * 4 + 2], sigma_ts = coef[g * 4 + 3];
-  __shared__ float red[9][4];
+  const float alpha_s = coef[0], sigma_s = coef[1], alpha_ts = coef[2], sigma_ts = coef[3];
   float n1[3];
   joint_noise_mean(nx1, sp, NL, red, n1);
   auto zk_lig = [&](int idx, int c, int i) {
@@ -640,15 +662,24 @@ __global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
   }
   if (nx3) {
     block_sum(s, 3, red);
-    const float m0 = s[0] / sp.n, m1 = s[1] / sp.n, m2 = s[2] / sp.n;
+    const float m[3] = {s[0] / sp.n, s[1] / sp.n, s[2] / sp.n};
     __syncthreads();
-    for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
-      z_lig[(size_t)i * D] -= m0; z_lig[(size_t)i * D + 1] -= m1; z_lig[(size_t)i * D + 2] -= m2;
-    }
-    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
-      z_poc[(size_t)i * DR] -= m0; z_poc[(size_t)i * DR + 1] -= m1; z_poc[(size_t)i * DR + 2] -= m2;
-    }
+    sub_rows3(z_lig, sp.l0, sp.l1, D, m);
+    sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
+    if (h_lig) { sub_rows3(h_lig, sp.l0, sp.l1, D, m); sub_rows3(h_poc, sp.p0, sp.p1, DR, m); }
   }
+}
+
+// dsb_ddpm_joint_inpaint_update: the joint RePaint iteration after the reverse step.
+__global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
+    float* z_lig, float* z_poc, const float* __restrict__ x0_lig, const float* __restrict__ x0_poc, const float* __restrict__ fix_lig,
+    const float* __restrict__ fix_poc, const float* __restrict__ nx1, const float* __restrict__ nhl1, const float* __restrict__ nhp1,
+    const float* __restrict__ nx3, const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* __restrict__ coef,
+    const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R) {
+  __shared__ float red[9][4];
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
+  repaint_joint(z_lig, z_poc, nullptr, nullptr, x0_lig, x0_poc, fix_lig, fix_poc, nx1, nhl1, nhp1, nx3, nhl3, nhp3,
+                coef + blockIdx.x * 4, sp, NL, A, R, red);
 }
 
 
@@ -693,18 +724,12 @@ __global__ void __launch_bounds__(128) ddpm_multistep_kernel(float* z_lig, float
   }
   block_sum(s, 3, red);
   const float cnt = joint ? sp.n : ((sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f);
-  const float m0 = s[0] / cnt, m1 = s[1] / cnt, m2 = s[2] / cnt;
+  const float m[3] = {s[0] / cnt, s[1] / cnt, s[2] / cnt};
   __syncthreads();
-  for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
-    const size_t r = (size_t)i * D;
-    z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
-    h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
-  }
-  for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
-    const size_t r = (size_t)i * DR;
-    z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
-    if (joint) { h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2; }
-  }
+  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(h_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
+  if (joint) sub_rows3(h_poc, sp.p0, sp.p1, DR, m);
 }
 
 
@@ -721,105 +746,32 @@ __device__ __forceinline__ float multistep_repaint_elem(float* z, float* hist, c
   return v;
 }
 
-// Conditional model: the 2M step with its ligand-COM removal, then ddpm_inpaint_kernel's iteration on its output.  Every
-// translation of the pocket coordinates is applied to the history too, so that the history stays in the pocket's frame.
+// Conditional model: the 2M step with its ligand-COM removal, which moves the pocket and the history too, then repaint_cond
+// with the history.
 __device__ __forceinline__ void multistep_repaint_cond(float* z, float* pocket, float* hist, const float* __restrict__ eps,
                                                        const float* __restrict__ known, const float* __restrict__ com_pocket0,
                                                        const float* __restrict__ fixed, const float* __restrict__ noise1,
                                                        const float* __restrict__ noise2, const float* k, const JointSpan& sp,
                                                        int A, int R, int commit, float (*red)[4]) {
-  const int g = blockIdx.x, l0 = sp.l0, l1 = sp.l1, p0 = sp.p0, p1 = sp.p1;
   const int D = 3 + A, DR = 3 + R;
-  const float alpha_s = k[5], sigma_s = k[6], alpha_ts = k[7], sigma_ts = k[8];
-  const float nl = (l1 - l0) > 0 ? (float)(l1 - l0) : 1.f, np_ = (p1 - p0) > 0 ? (float)(p1 - p0) : 1.f;
-  float v[9] = {0.f, 0.f, 0.f};
-  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
+  const float nl = (sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f;
+  float v[3] = {0.f, 0.f, 0.f};
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
     const float o = multistep_repaint_elem(z, hist, eps, (size_t)idx, k, commit);
     const int c = idx % D;
     if (c < 3) v[c] += o;
   }
   block_sum(v, 3, red);
   const float m[3] = {v[0] / nl, v[1] / nl, v[2] / nl};
-  for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
-    const size_t r = (size_t)i * D;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) { z[r + c] -= m[c]; hist[r + c] -= m[c]; }
-  }
-  for (int i = p0 + threadIdx.x; i < p1; i += blockDim.x) {
-    const size_t r = (size_t)i * DR;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) pocket[r + c] -= m[c];
-  }
+  sub_rows3(z, sp.l0, sp.l1, D, m);
+  sub_rows3(hist, sp.l0, sp.l1, D, m);
+  sub_rows3(pocket, sp.p0, sp.p1, DR, m);
   __syncthreads();                      // z = z_unknown and the moved pocket are complete
-
-  // from here on ddpm_inpaint_kernel, with the history following the pocket
-  v[0] = v[1] = v[2] = 0.f;
-  for (int i = p0 + threadIdx.x; i < p1; i += blockDim.x) {
-    v[0] += pocket[(size_t)i * DR + 0]; v[1] += pocket[(size_t)i * DR + 1]; v[2] += pocket[(size_t)i * DR + 2];
-  }
-  block_sum(v, 3, red);
-  float shift[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) shift[c] = v[c] / np_ - com_pocket0[g * 3 + c];
-  auto zk_raw = [&](int idx, int c) {
-    const float xk = c < 3 ? known[idx] + shift[c] : known[idx];
-    return alpha_s * xk + sigma_s * noise1[idx];
-  };
-  v[0] = v[1] = v[2] = 0.f;
-  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
-    const int c = idx % D;
-    if (c < 3) v[c] += zk_raw(idx, c);
-  }
-  block_sum(v, 3, red);
-  const float comk[3] = {v[0] / nl, v[1] / nl, v[2] / nl};
-  for (int q = 0; q < 7; ++q) v[q] = 0.f;
-  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
-    const int c = idx % D, i = idx / D;
-    if (c < 3 && fixed[i] != 0.f) { v[c] += zk_raw(idx, c) - comk[c]; v[3 + c] += z[idx]; if (c == 0) v[6] += 1.f; }
-  }
-  block_sum(v, 7, red);
-  const float nf = v[6] > 0.f ? v[6] : 1.f;
-  float dx[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) dx[c] = v[3 + c] / nf - v[c] / nf;
-  float s2[3] = {0.f, 0.f, 0.f};
-  for (int idx = l0 * D + threadIdx.x; idx < l1 * D; idx += blockDim.x) {
-    const int c = idx % D, i = idx / D;
-    float zk = zk_raw(idx, c);
-    if (c < 3) zk = (zk - comk[c]) + dx[c];
-    const float f = fixed[i];
-    float o = zk * f + z[idx] * (1.f - f);
-    if (noise2) { o = alpha_ts * o + sigma_ts * noise2[idx]; if (c < 3) s2[c] += o; }
-    z[idx] = o;
-  }
-  float com2[3] = {0.f, 0.f, 0.f};
-  if (noise2) {
-    block_sum(s2, 3, red);
-#pragma unroll
-    for (int c = 0; c < 3; ++c) com2[c] = s2[c] / nl;
-    __syncthreads();
-  }
-  for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
-    const size_t r = (size_t)i * D;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float h = (hist[r + c] - comk[c]) + dx[c];
-      if (noise2) { h -= com2[c]; z[r + c] -= com2[c]; }
-      hist[r + c] = h;
-    }
-  }
-  for (int idx = p0 * DR + threadIdx.x; idx < p1 * DR; idx += blockDim.x) {
-    const int c = idx % DR;
-    if (c < 3) {
-      float q = (pocket[idx] - comk[c]) + dx[c];
-      if (noise2) q -= com2[c];
-      pocket[idx] = q;
-    }
-  }
+  repaint_cond(z, pocket, hist, known, com_pocket0, fixed, noise1, noise2, k + 5, sp, A, R, red);
 }
 
-// Joint model: the 2M step of ligand and pocket with the joint COM removal, then ddpm_joint_inpaint_kernel's iteration.  The
-// blend keeps the frame of the unknown part; the jump back's COM removal moves the history with z.
+// Joint model: the 2M step of ligand and pocket with the joint COM removal, which moves the history too, then repaint_joint
+// with the history.
 __device__ __forceinline__ void multistep_repaint_joint(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
                                                         const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
                                                         const float* __restrict__ x0_lig, const float* __restrict__ x0_poc,
@@ -830,8 +782,7 @@ __device__ __forceinline__ void multistep_repaint_joint(float* z_lig, float* z_p
                                                         const float* k, const JointSpan& sp, int NL, int A, int R, int commit,
                                                         float (*red)[4]) {
   const int D = 3 + A, DR = 3 + R;
-  const float alpha_s = k[5], sigma_s = k[6], alpha_ts = k[7], sigma_ts = k[8];
-  float v[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  float v[3] = {0.f, 0.f, 0.f};
   for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
     const float o = multistep_repaint_elem(z_lig, h_lig, eps_lig, (size_t)idx, k, commit);
     const int c = idx % D;
@@ -843,90 +794,14 @@ __device__ __forceinline__ void multistep_repaint_joint(float* z_lig, float* z_p
     if (c < 3) v[c] += o;
   }
   block_sum(v, 3, red);
-  {
-    const float m0 = v[0] / sp.n, m1 = v[1] / sp.n, m2 = v[2] / sp.n;
-    for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
-      const size_t r = (size_t)i * D;
-      z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
-      h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
-    }
-    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
-      const size_t r = (size_t)i * DR;
-      z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
-      h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2;
-    }
-  }
+  const float m[3] = {v[0] / sp.n, v[1] / sp.n, v[2] / sp.n};
+  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(h_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
+  sub_rows3(h_poc, sp.p0, sp.p1, DR, m);
   __syncthreads();                      // z = the unknown part, complete
-
-  // from here on ddpm_joint_inpaint_kernel, with the history following z through the jump back
-  float n1[3];
-  joint_noise_mean(nx1, sp, NL, red, n1);
-  auto zk_lig = [&](int idx, int c, int i) {
-    const float e = c < 3 ? nx1[(size_t)i * 3 + c] - n1[c] : nhl1[(size_t)i * A + (c - 3)];
-    return alpha_s * x0_lig[idx] + sigma_s * e;
-  };
-  auto zk_poc = [&](int idx, int c, int i) {
-    const float e = c < 3 ? nx1[(size_t)(NL + i) * 3 + c] - n1[c] : nhp1[(size_t)i * R + (c - 3)];
-    return alpha_s * x0_poc[idx] + sigma_s * e;
-  };
-  for (int q = 0; q < 7; ++q) v[q] = 0.f;
-  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const int c = idx % D, i = idx / D;
-    if (c < 3 && fix_lig[i] != 0.f) { v[c] += z_lig[idx]; v[3 + c] += zk_lig(idx, c, i); if (c == 0) v[6] += 1.f; }
-  }
-  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
-    const int c = idx % DR, i = idx / DR;
-    if (c < 3 && fix_poc[i] != 0.f) { v[c] += z_poc[idx]; v[3 + c] += zk_poc(idx, c, i); if (c == 0) v[6] += 1.f; }
-  }
-  block_sum(v, 7, red);
-  const float nf = v[6] > 0.f ? v[6] : 1.f;
-  float shift[3];
-#pragma unroll
-  for (int c = 0; c < 3; ++c) shift[c] = v[c] / nf - v[3 + c] / nf;
-  float n3[3] = {0.f, 0.f, 0.f};
-  if (nx3) joint_noise_mean(nx3, sp, NL, red, n3);
-  float s[3] = {0.f, 0.f, 0.f};
-  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const int c = idx % D, i = idx / D;
-    float zk = zk_lig(idx, c, i);
-    if (c < 3) zk += shift[c];
-    const float f = fix_lig[i];
-    float o = zk * f + z_lig[idx] * (1.f - f);
-    if (nx3) {
-      const float e = c < 3 ? nx3[(size_t)i * 3 + c] - n3[c] : nhl3[(size_t)i * A + (c - 3)];
-      o = alpha_ts * o + sigma_ts * e;
-      if (c < 3) s[c] += o;
-    }
-    z_lig[idx] = o;
-  }
-  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
-    const int c = idx % DR, i = idx / DR;
-    float zk = zk_poc(idx, c, i);
-    if (c < 3) zk += shift[c];
-    const float f = fix_poc[i];
-    float o = zk * f + z_poc[idx] * (1.f - f);
-    if (nx3) {
-      const float e = c < 3 ? nx3[(size_t)(NL + i) * 3 + c] - n3[c] : nhp3[(size_t)i * R + (c - 3)];
-      o = alpha_ts * o + sigma_ts * e;
-      if (c < 3) s[c] += o;
-    }
-    z_poc[idx] = o;
-  }
-  if (nx3) {
-    block_sum(s, 3, red);
-    const float m0 = s[0] / sp.n, m1 = s[1] / sp.n, m2 = s[2] / sp.n;
-    __syncthreads();
-    for (int i = sp.l0 + threadIdx.x; i < sp.l1; i += blockDim.x) {
-      const size_t r = (size_t)i * D;
-      z_lig[r] -= m0; z_lig[r + 1] -= m1; z_lig[r + 2] -= m2;
-      h_lig[r] -= m0; h_lig[r + 1] -= m1; h_lig[r + 2] -= m2;
-    }
-    for (int i = sp.p0 + threadIdx.x; i < sp.p1; i += blockDim.x) {
-      const size_t r = (size_t)i * DR;
-      z_poc[r] -= m0; z_poc[r + 1] -= m1; z_poc[r + 2] -= m2;
-      h_poc[r] -= m0; h_poc[r + 1] -= m1; h_poc[r + 2] -= m2;
-    }
-  }
+  repaint_joint(z_lig, z_poc, h_lig, h_poc, x0_lig, x0_poc, fix_lig, fix_poc, nx1, nhl1, nhp1, nx3, nhl3, nhp3, k + 5, sp, NL,
+                A, R, red);
 }
 
 // One block per graph; coef row g = the 2M row (5) then the RePaint row (4).

@@ -841,16 +841,21 @@ class EnVariationalDiffusion(nn.Module):
 
     def _joint_fast_inpaint_step(self, s, i, t, row, gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket, lig_fixed,
                                  pocket_fixed, lsel, psel, lmask, pmask, sampler, eta, commit):
-        """Eager RePaint iteration (s, block i) of the joint inpaint with the 'ddim' / 'dpmpp_2m' step (DESIGN §14), without
-        the jump back (_joint_renoise).  ``hist``: () for DDIM; for 2M (hist_lig, hist_pocket) = x0_hat committed by the last
-        iteration of step s + 1, in the frame of z.  The 2M COM removal moves it with z; the blend keeps the frame of the
-        unknown part, so nothing else moves it; ``commit``: this iteration's x0_hat becomes the history.  Returns
-        (z_lig, z_pocket, hist)."""
+        """Eager RePaint iteration (s, block i) of the joint inpaint (DESIGN §14), without the jump back (_joint_renoise): the
+        known part, the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row`` and t; 'ddim' / 'dpmpp_2m': the few-step
+        step with ``row`` [1, k], the step's row of _fast_tables), the COM alignment and the blend.  ``hist``: () for
+        'ddpm' and DDIM; for 2M (hist_lig, hist_pocket) = x0_hat committed by the last iteration of step s + 1, in the frame
+        of z.  The 2M COM removal moves it with z; the blend keeps the frame of the unknown part, so nothing else moves it;
+        ``commit``: this iteration's x0_hat becomes the history.  Returns (z_lig, z_pocket, hist)."""
         from . import seeded
         nd = self.n_dims
+        # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
         self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_KNOWN)
         zk_lig, zk_pocket, _, _ = self.noised_representation(xh0_lig, xh0_pocket, lmask, pmask, gamma_s)
-        if sampler == 'ddim':
+        if sampler == 'ddpm':
+            self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_REVERSE)
+            zu_lig, zu_pocket = self.sample_p_zs_given_zt(row, t, z_lig, z_pocket, lmask, pmask)
+        elif sampler == 'ddim':
             zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, None, None, lmask, pmask, sampler, eta, i)
         else:
             c = row.expand(t.shape[0], -1)
@@ -866,7 +871,7 @@ class EnVariationalDiffusion(nn.Module):
             for x, m in ((zu_lig, lmask), (zu_pocket, pmask), (x0_l, lmask), (x0_p, pmask), (hl, lmask), (hp, pmask)):
                 x[:, :nd] -= mean[m]
             hist = (x0_l, x0_p) if commit else (hl, hp)
-        # the rest is _inpaint's iteration
+        # align the COM of the noised known part with the denoised one (en_diffusion.py:751-772)
         shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
             self._fixed_com(zk_lig[:, :nd], zk_pocket[:, :nd], lsel, psel, lmask, pmask)
         zk_lig[:, :nd] = zk_lig[:, :nd] + shift[lmask]
@@ -876,7 +881,10 @@ class EnVariationalDiffusion(nn.Module):
         return z_lig, z_pocket, hist
 
     def _joint_renoise(self, z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask):
-        """sample_p_zt_given_zs (the jump back) with the 2M history ``hist`` (or ()) moved by the same joint COM removal."""
+        """sample_p_zt_given_zs (the jump back, en_diffusion.py:790-807) with the 2M history ``hist`` (or ()) moved by the same
+        joint COM removal."""
+        if not hist:
+            return (*self.sample_p_zt_given_zs(z_lig, z_pocket, lmask, pmask, gamma_t, gamma_s), ())
         nd = self.n_dims
         _, sigma_ts, alpha_ts = self.sigma_and_alpha_t_given_s(gamma_t, gamma_s, z_lig)
         zl, zp = self.sample_normal(alpha_ts[lmask] * z_lig, alpha_ts[pmask] * z_pocket, sigma_ts, lmask, pmask)
@@ -1081,12 +1089,10 @@ class EnVariationalDiffusion(nn.Module):
                                 t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
                                 g_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
                                 g_s = self.inflate_batch_array(self.gamma(s_arr), ligand['x'])
-                                if two_m:
-                                    zl, zp, hist = self._joint_renoise(st['zl'], st['zp'], st['hist'], g_t, g_s, lmask, pmask)
-                                    for x, y in zip(st['hist'], hist):
-                                        x.copy_(y)
-                                else:
-                                    zl, zp = self.sample_p_zt_given_zs(st['zl'], st['zp'], lmask, pmask, g_t, g_s)
+                                hist = st.get('hist', ())
+                                zl, zp, moved = self._joint_renoise(st['zl'], st['zp'], hist, g_t, g_s, lmask, pmask)
+                                for x, y in zip(hist, moved):
+                                    x.copy_(y)
                                 st['zl'].copy_(zl); st['zp'].copy_(zp); st['step'].add_(jump_length)
                                 if st['seeded']:
                                     st['u'].add_(1)
@@ -1097,17 +1103,21 @@ class EnVariationalDiffusion(nn.Module):
             dyn.check_status()
             z_lig, z_pocket = st['zl'].clone(), st['zp'].clone()
             self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :nd], z_pocket[:, :nd]), dim=0), combined_mask)
-        elif sampler != 'ddpm':
-            t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
+        else:
+            if sampler != 'ddpm':
+                t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
             hist = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket)) if sampler == 'dpmpp_2m' else ()
             for i, n_denoise in enumerate(schedule):
                 for j in range(n_denoise):
                     jump = j == n_denoise - 1 and i < len(schedule) - 1
-                    s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device) / timesteps
+                    s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
+                    t_array = (s_array + 1) / timesteps
+                    s_array = s_array / timesteps
                     gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
+                    t, row = (t_array, s_array) if sampler == 'ddpm' else (t_table[s].expand(n_samples, 1), coef[s:s + 1])
                     z_lig, z_pocket, hist = self._joint_fast_inpaint_step(
-                        s, i, t_table[s].expand(n_samples, 1), coef[s:s + 1], gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket,
-                        lig_fixed, pocket_fixed, lsel, psel, lmask, pmask, sampler, eta, not jump)
+                        s, i, t, row, gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket, lig_fixed, pocket_fixed, lsel, psel,
+                        lmask, pmask, sampler, eta, not jump)
                     self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :nd], z_pocket[:, :nd]), dim=0), combined_mask)
                     if (n_denoise > jump_length or i == len(schedule) - 1) and (s * return_frames) % timesteps == 0:
                         idx = (s * return_frames) // timesteps
@@ -1118,40 +1128,6 @@ class EnVariationalDiffusion(nn.Module):
                         self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
                         z_lig, z_pocket, hist = self._joint_renoise(z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask)
                         s = s + jump_length
-                    s -= 1
-        else:
-            for i, n_denoise in enumerate(schedule):
-                for j in range(n_denoise):
-                    s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
-                    t_array = (s_array + 1) / timesteps
-                    s_array = s_array / timesteps
-                    gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
-                    # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
-                    self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_KNOWN)
-                    zk_lig, zk_pocket, _, _ = self.noised_representation(xh0_lig, xh0_pocket, lmask, pmask, gamma_s)
-                    self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_REVERSE)
-                    zu_lig, zu_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, z_pocket, lmask, pmask)
-                    # align the COM of the noised known part with the denoised one (en_diffusion.py:751-772)
-                    shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
-                        self._fixed_com(zk_lig[:, :nd], zk_pocket[:, :nd], lsel, psel, lmask, pmask)
-                    zk_lig[:, :nd] = zk_lig[:, :nd] + shift[lmask]
-                    zk_pocket[:, :nd] = zk_pocket[:, :nd] + shift[pmask]
-                    z_lig = zk_lig * lig_fixed + zu_lig * (1 - lig_fixed)
-                    z_pocket = zk_pocket * pocket_fixed + zu_pocket * (1 - pocket_fixed)
-                    self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :nd], z_pocket[:, :nd]), dim=0), combined_mask)
-
-                    if (n_denoise > jump_length or i == len(schedule) - 1) and (s * return_frames) % timesteps == 0:
-                        idx = (s * return_frames) // timesteps
-                        out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
-
-                    if j == n_denoise - 1 and i < len(schedule) - 1:      # jump back jump_length steps (en_diffusion.py:790-807)
-                        t = s + jump_length
-                        t_back = torch.full((n_samples, 1), fill_value=t, device=z_lig.device) / timesteps
-                        gamma_s = self.inflate_batch_array(self.gamma(s_array), ligand['x'])
-                        gamma_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
-                        self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_RENOISE)
-                        z_lig, z_pocket = self.sample_p_zt_given_zs(z_lig, z_pocket, lmask, pmask, gamma_t, gamma_s)
-                        s = t
                     s -= 1
 
         self._draw_at(seeded.STAGE_FINAL)
