@@ -18,7 +18,8 @@ EXPORTED_SYMBOLS = (
     'dsb_edge_capacity', 'dsb_dynamics_workspace_bytes', 'dsb_dynamics_forward', 'dsb_dynamics_edges',
     'dsb_dynamics_last_launch_count', 'dsb_set_programmatic_launch', 'dsb_dynamics_set_math_mode', 'dsb_dynamics_set_deterministic', 'dsb_dynamics_set_profiling', 'dsb_dynamics_collect_profile',
     'dsb_ddpm_ligand_update', 'dsb_ddpm_inpaint_update', 'dsb_ddpm_joint_update', 'dsb_ddpm_joint_inpaint_update', 'dsb_ddpm_noise',
-    'dsb_ddpm_multistep_update', 'dsb_ddpm_multistep_inpaint_update',
+    'dsb_ddpm_multistep_update', 'dsb_ddpm_multistep_inpaint_update', 'dsb_ddpm_multistep3_update',
+    'dsb_ddpm_multistep3_inpaint_update',
     'dsb_ddpm_vlb_terms', 'dsb_last_error', 'dsb_version', 'dsb_dynamics_set_stop_after', 'dsb_workspace_region',
     'dsb_seeded_normal',
 )
@@ -116,6 +117,10 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     lib.dsb_ddpm_multistep_update.restype = C.c_int
     lib.dsb_ddpm_multistep_inpaint_update.argtypes = [vp] * 20 + [i64, i64, i64, i32, i32, i32, i32, vp]
     lib.dsb_ddpm_multistep_inpaint_update.restype = C.c_int
+    lib.dsb_ddpm_multistep3_update.argtypes = [vp] * 11 + [i64, i64, i64, i32, i32, i32, vp]
+    lib.dsb_ddpm_multistep3_update.restype = C.c_int
+    lib.dsb_ddpm_multistep3_inpaint_update.argtypes = [vp] * 22 + [i64, i64, i64, i32, i32, i32, i32, vp]
+    lib.dsb_ddpm_multistep3_inpaint_update.restype = C.c_int
     lib.dsb_ddpm_noise.argtypes = [vp] * 7 + [i64, i64, i64, i32, i32, vp, vp, vp]
     lib.dsb_ddpm_noise.restype = C.c_int
     lib.dsb_ddpm_vlb_terms.argtypes = [vp] * 16 + [i64, i64, i64, i32, i32, C.c_float, C.c_float, i32, vp, vp, vp]

@@ -25,8 +25,8 @@ import torch.nn.functional as F
 
 from . import _native, seeded
 from .dynamics import EGNNDynamics
-from .en_diffusion import (EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, scatter_add, scatter_mean,
-                           num_nodes_to_batch_mask)
+from .en_diffusion import (MULTISTEP, EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, multistep3_update,
+                           scatter_add, scatter_mean, num_nodes_to_batch_mask)
 
 
 class ConditionalDDPM(EnVariationalDiffusion):
@@ -173,10 +173,13 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 st.update(fast_t=fast_t, fast_table=fast, coef_fast=torch.zeros((n_samples, fast.shape[1]), device=device),
                           eta=eta, sampler=sampler)
                 st['noise'].zero_()
-                if sampler == 'dpmpp_2m':   # RePaint rounds: the 2M row and the RePaint row in one [n, 9] buffer
+                if sampler in MULTISTEP:   # RePaint rounds: the 2M / 3M row and the RePaint row in one [n, 9 | 10] buffer
                     st['hist'] = torch.zeros_like(z_lig)
-                    st.update(ms_table=torch.cat((fast, coef_table[:, 3:]), 1).contiguous(),
-                              coef9=torch.zeros((n_samples, 9), device=device))
+                    if sampler == 'dpmpp_3m':
+                        st['hist2'] = torch.zeros_like(z_lig)
+                    ms = torch.cat((fast, coef_table[:, 3:]), 1).contiguous()
+                    st['ms_table'] = ms
+                    st['coef9' if sampler == 'dpmpp_2m' else 'coef10'] = torch.zeros((n_samples, ms.shape[1]), device=device)
             self._graph_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -186,9 +189,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def _captured_step(self, st, kind):
         """One iteration as a python callable over the static buffers of ``st``.
         kind: 'reverse' (z_t -> z_s, step -= 1) | 'inpaint_renoise' (reverse step + RePaint blend + re-noise to t) |
-        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' (_fast_captured_step).  The inpainting kinds
+        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' | 'dpmpp_3m' (_fast_captured_step).  The inpainting kinds
         of an engine built for a few-step sampler are _fast_inpaint_captured_step."""
-        if kind in ('ddim', 'dpmpp_2m'):
+        if kind in ('ddim',) + MULTISTEP:
             return self._fast_captured_step(st, kind)
         if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
             return self._fast_inpaint_captured_step(st, kind)
@@ -249,8 +252,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
         st['z'].copy_(z_lig); st['pocket'].copy_(xh_pocket); st['step'].fill_(first_s)
         if st['seeded']:
             st['u'].zero_()
-        if 'hist' in st:
-            st['hist'].zero_()
+        for key in ('hist', 'hist2'):
+            if key in st:
+                st[key].zero_()
 
     def _graph(self, st, kind, z_lig, xh_pocket, first_s):
         """Captured CUDA graph of ``kind`` (captured on first use; capture leaves the static state as it found it)."""
@@ -304,9 +308,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return st['z'].clone(), st['pocket'].clone()
 
     def _fast_captured_step(self, st, kind):
-        """One 'ddim' or 'dpmpp_2m' step over the static buffers of ``st`` (step -= 1): table row of the step counter ->
-        native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0) or
-        dsb_ddpm_multistep_update."""
+        """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step over the static buffers of ``st`` (step -= 1): table row of the step
+        counter -> native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0),
+        dsb_ddpm_multistep_update or dsb_ddpm_multistep3_update."""
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
@@ -330,19 +334,24 @@ class ConditionalDDPM(EnVariationalDiffusion):
                     st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef_fast'].data_ptr(), lm.data_ptr(),
                     pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, st['z'].data_ptr(),
                     st['pocket'].data_ptr(), stream))
-            else:
+            elif kind == 'dpmpp_2m':
                 _native.check(lib.dsb_ddpm_multistep_update(
                     st['z'].data_ptr(), st['pocket'].data_ptr(), st['hist'].data_ptr(), None, eps.data_ptr(), None,
                     st['coef_fast'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, 0,
                     stream))
+            else:
+                _native.check(lib.dsb_ddpm_multistep3_update(
+                    st['z'].data_ptr(), st['pocket'].data_ptr(), st['hist'].data_ptr(), None, st['hist2'].data_ptr(), None,
+                    eps.data_ptr(), None, st['coef_fast'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf,
+                    self.residue_nf, 0, stream))
             st['step'].sub_(1)
         return run
 
     def _graphed_fast_loop(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta, return_frames,
                            out_lig, out_pocket, top=None):
-        """The whole 'ddim' / 'dpmpp_2m' reverse loop as ``timesteps`` replays of one captured step; frames are copied from
-        the static state between replays, so the history of the multistep sampler runs through them.  ``top``: the grid's
-        top t as _fast_tables takes it (diversify)."""
+        """The whole 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' reverse loop as ``timesteps`` replays of one captured step; frames are
+        copied from the static state between replays, so the history of the multistep samplers runs through them.  ``top``:
+        the grid's top t as _fast_tables takes it (diversify)."""
         dyn: EGNNDynamics = self.dynamics
         st = self._engine(z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, self._seeds(), sampler, eta, top)
         s0 = timesteps - 1
@@ -362,9 +371,10 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return st['z'].clone(), st['pocket'].clone()
 
     def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta, u=0):
-        """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s (DESIGN §13); ``row`` [1, k]: the step's row of _fast_tables.  Returns
-        (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M only), in the frame of the returned z.  ``u``: the
-        resampling round of the seeded DDIM draw (RePaint)."""
+        """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s (DESIGN §13, §15); ``row`` [1, k]: the step's row of
+        _fast_tables.  Returns (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M), or the pair (m1, m2) of x0_hat
+        of this step and of the one before it (3M), in the frame of the returned z.  ``u``: the resampling round of the seeded
+        DDIM draw (RePaint)."""
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
         cl = c[lig_mask]
@@ -379,6 +389,15 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 mu[:, :nd], xh_pocket[:, :nd] = self.remove_mean_batch(mu[:, :nd], xh_pocket[:, :nd], lig_mask, pocket_mask)
                 z_lig = mu
             return z_lig, xh_pocket, hist
+        if sampler == 'dpmpp_3m':
+            # the ligand COM leaves z, the pocket and both histories together
+            NP, NL = xh_pocket.shape[0], z_lig.shape[0]
+            z_lig, x0, m2 = multistep3_update(z_lig, eps, *hist, cl)
+            xh_pocket = xh_pocket.clone()
+            z_lig[:, :nd], moved = self.remove_mean_batch(z_lig[:, :nd], torch.cat((xh_pocket[:, :nd], x0[:, :nd], m2[:, :nd])),
+                                                          lig_mask, torch.cat((pocket_mask, lig_mask, lig_mask)))
+            xh_pocket[:, :nd], x0[:, :nd], m2[:, :nd] = moved[:NP], moved[NP:NP + NL], moved[NP + NL:]
+            return z_lig, xh_pocket, (x0, m2)
         x0 = (z_lig - cl[:, 3:4] * eps) * cl[:, 2:3]
         z_lig = cl[:, 0:1] * z_lig + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0 - cl[:, 4:5] * hist)
         # the ligand COM leaves z, the pocket and the history together (one mean, subtracted from both)
@@ -390,16 +409,18 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return z_lig, xh_pocket, x0
 
     def _fast_inpaint_captured_step(self, st, kind):
-        """One RePaint round of an engine built for 'ddim' or 'dpmpp_2m' (DESIGN §14); kind as _captured_step
+        """One RePaint round of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15); kind as _captured_step
         ('inpaint_renoise': re-noised, the round does not commit; 'inpaint_last': the last round of the step, which commits
-        its x0_hat as the 2M history).  DDIM: native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients ->
-        dsb_ddpm_inpaint_update.  2M: native denoiser -> dsb_ddpm_multistep_inpaint_update."""
+        its x0_hat as the 2M / 3M history).  DDIM: native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients ->
+        dsb_ddpm_inpaint_update.  2M: native denoiser -> dsb_ddpm_multistep_inpaint_update.  3M: native denoiser ->
+        dsb_ddpm_multistep3_inpaint_update."""
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
         NL, NP = st['z'].shape[0], st['pocket'].shape[0]
         renoise = kind == 'inpaint_renoise'
         ddim = st['sampler'] == 'ddim'
+        ms_key = 'coef9' if st['sampler'] == 'dpmpp_2m' else 'coef10'      # the 2M / 3M row + the RePaint row
 
         def draw(out, purpose):
             if st['seeded']:
@@ -418,7 +439,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
                 st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
             else:
-                st['coef9'].copy_(st['ms_table'].index_select(0, idx).expand(n, 9))
+                st[ms_key].copy_(st['ms_table'].index_select(0, idx).expand(n, st['ms_table'].shape[1]))
             eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
             if ddim and st['eta'] > 0:
                 draw(st['noise'], seeded.PURPOSE_REVERSE)
@@ -434,11 +455,16 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 _native.check(lib.dsb_ddpm_inpaint_update(
                     ptr(st['z']), ptr(st['pocket']), ptr(ip['known']), ptr(ip['com0']), ptr(ip['fixed']), ptr(st['noise1']), n2,
                     ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            else:
+            elif st['sampler'] == 'dpmpp_2m':
                 _native.check(lib.dsb_ddpm_multistep_inpaint_update(
                     ptr(st['z']), ptr(st['pocket']), ptr(st['hist']), None, ptr(eps), None, ptr(ip['known']), None,
-                    ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None, ptr(st['coef9']),
+                    ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None, ptr(st[ms_key]),
                     ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 0, int(not renoise), stream))
+            else:
+                _native.check(lib.dsb_ddpm_multistep3_inpaint_update(
+                    ptr(st['z']), ptr(st['pocket']), ptr(st['hist']), None, ptr(st['hist2']), None, ptr(eps), None,
+                    ptr(ip['known']), None, ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None,
+                    ptr(st[ms_key]), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 0, int(not renoise), stream))
             if renoise:
                 if st['seeded']:
                     st['u'].add_(1)
@@ -451,10 +477,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def _fast_inpaint_step(self, s, u, t, row, gamma_s, gamma_t, z_lig, xh_pocket, hist, ligand_x, xh_ligand, com_pocket_0,
                            lig_fixed, lmask, pmask, sampler, eta, last):
         """Eager RePaint round (s, u) of _inpaint (DESIGN §14): the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row``
-        and t; 'ddim' / 'dpmpp_2m': the few-step step with ``row`` [1, k], the step's row of _fast_tables), then the known
-        part, the COM alignment, the blend and, unless ``last``, the re-noising.  2M: ``hist`` is x0_hat committed by the
-        last round of step s + 1, kept in the pocket's frame: every translation of the pocket coordinates moves it too, and
-        the last round of step s commits its own x0_hat.  Returns (z_lig, xh_pocket, hist)."""
+        and t; 'ddim' / 'dpmpp_2m' / 'dpmpp_3m': the few-step step with ``row`` [1, k], the step's row of _fast_tables), then
+        the known part, the COM alignment, the blend and, unless ``last``, the re-noising.  2M: ``hist`` is x0_hat committed
+        by the last round of step s + 1, kept in the pocket's frame: every translation of the pocket coordinates moves it
+        too, and the last round of step s commits its own x0_hat.  3M: ``hist`` is the pair (m1, m2) under the same rule; the
+        commit is m2 <- m1, m1 <- x0_hat.  Returns (z_lig, xh_pocket, hist)."""
         nd, NL, NP = self.n_dims, z_lig.shape[0], xh_pocket.shape[0]
         fixed_rows = lig_fixed.bool().view(-1)
         if sampler == 'ddpm':
@@ -462,18 +489,24 @@ class ConditionalDDPM(EnVariationalDiffusion):
             z_unknown, xh_pocket = self.sample_p_zs_given_zt(row, t, z_lig, xh_pocket, lmask, pmask)
         elif sampler == 'ddim':
             z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u)
-        if sampler != 'dpmpp_2m':
+        if sampler not in MULTISTEP:
             # only the x columns of the pocket are ever translated
             frame, fmask = xh_pocket[:, :nd], pmask
         else:
             c = row.expand(t.shape[0], -1)[lmask]
             eps, _ = self.dynamics(z_lig, xh_pocket, t, lmask, pmask)
-            x0 = (z_lig - c[:, 3:4] * eps) * c[:, 2:3]
-            z_unknown = c[:, 0:1] * z_lig + c[:, 1:2] * ((1 + c[:, 4:5]) * x0 - c[:, 4:5] * hist)
-            # frame: the rows that every pocket translation moves (pocket, history, x0_hat), under the pocket's graph index
-            fmask = torch.cat((pmask, lmask, lmask))
+            if sampler == 'dpmpp_2m':
+                x0 = (z_lig - c[:, 3:4] * eps) * c[:, 2:3]
+                z_unknown = c[:, 0:1] * z_lig + c[:, 1:2] * ((1 + c[:, 4:5]) * x0 - c[:, 4:5] * hist)
+                hists = (hist,)
+            else:           # (m1, m2, and the m2 a commit would write)
+                z_unknown, x0, m2_next = multistep3_update(z_lig, eps, *hist, c)
+                hists = hist + (m2_next,)
+            # frame: the rows that every pocket translation moves (pocket, histories, x0_hat), under the pocket's graph index
+            fmask = torch.cat((pmask,) + (lmask,) * (len(hists) + 1))
             z_unknown[:, :nd], frame = self.remove_mean_batch(
-                z_unknown[:, :nd], torch.cat((xh_pocket[:, :nd], hist[:, :nd], x0[:, :nd])), lmask, fmask)
+                z_unknown[:, :nd], torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hists) + (x0[:, :nd],)), lmask,
+                fmask)
 
         # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
         com_pocket = scatter_mean(frame[:NP], pmask, dim=0)
@@ -495,6 +528,10 @@ class ConditionalDDPM(EnVariationalDiffusion):
             keep = x0 if last else hist
             rows = frame[NP + NL:] if last else frame[NP:NP + NL]
             hist = torch.cat((rows, keep[:, nd:]), dim=1)
+        elif sampler == 'dpmpp_3m':
+            keep = (x0, m2_next) if last else hist
+            rows = (frame[NP + 3 * NL:], frame[NP + 2 * NL:NP + 3 * NL]) if last else (frame[NP:NP + NL], frame[NP + NL:NP + 2 * NL])
+            hist = tuple(torch.cat((r, k[:, nd:]), dim=1) for r, k in zip(rows, keep))
         return z_lig, xh_pocket, hist
 
     def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,
@@ -534,7 +571,8 @@ class ConditionalDDPM(EnVariationalDiffusion):
     def sample_given_pocket(self, pocket, num_nodes_lig, return_frames=1, timesteps=None, seeds=None, sampler='ddpm', eta=0.0):
         """conditional_model.py:479-555.  ``seeds``: one int64 per sample (seeded.py); every draw then comes from the
         sample's own seed instead of torch's global generator.  ``sampler``: 'ddpm' (the reference's ancestral step),
-        'ddim' (with noise level ``eta`` in [0, 1]) or 'dpmpp_2m', on the same ``timesteps`` grid (DESIGN §13)."""
+        'ddim' (with noise level ``eta`` in [0, 1]), 'dpmpp_2m' or 'dpmpp_3m', on the same ``timesteps`` grid (DESIGN §13,
+        §15)."""
         check_sampler(sampler, eta)
         timesteps = self.T if timesteps is None else timesteps
         assert 0 < return_frames <= timesteps
@@ -571,7 +609,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
             self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
         elif sampler != 'ddpm':
             t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
-            hist = torch.zeros_like(z_lig)
+            hist = self._empty_history(z_lig, sampler)
             for s in reversed(range(0, timesteps)):
                 z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
                                                          hist, lig_mask, pocket['mask'], sampler, eta)
@@ -664,7 +702,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
         else:
             if sampler != 'ddpm':
                 t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
-            hist = torch.zeros_like(z_lig)
+            hist = self._empty_history(z_lig, sampler)
             for s in reversed(range(0, timesteps)):
                 for u in range(resamplings):
                     s_array = torch.full((n_samples, 1), fill_value=s, device=device)
@@ -832,7 +870,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
                                                        sampler, eta, 1, *frame, top=top)
         elif sampler != 'ddpm' and noising_steps > 0:
             t_table, coef = self._fast_tables(denoising_steps, sampler, eta, z_lig.device, top)
-            hist = torch.zeros_like(z_lig)
+            hist = self._empty_history(z_lig, sampler)
             for s in reversed(range(0, denoising_steps)):
                 z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
                                                          hist, lig_mask, pocket['mask'], sampler, eta)

@@ -440,13 +440,14 @@ __device__ __forceinline__ void block_sum(float* v, int nv, float (*red)[4]) {
 //   known part noised to level s around the pocket's current COM, ligand-COM removed (noised_representation, :162-183),
 //   COM of the fixed atoms aligned noised -> denoised (:645-656), blend (:659), and with noise2 the re-noising step
 //   z_t ~ q(z_t | z_s) with its own COM removal (sample_p_zt_given_zs, :420-430, :662-666).
-// coef = (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}).  hist (the 2M history, or null) takes every translation of the pocket
-// coordinates, so that it stays in the pocket's frame.  Every per-element fp32 operation is the one the torch ops of the
+// coef = (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}).  hist (the 2M history, or null) and hist2 (the second 3M history, or
+// null) take every translation of the pocket coordinates, so that they stay in the pocket's frame.  Every per-element fp32 operation is the one the torch ops of the
 // eager loop perform, in the same order; only the per-graph means are summed in a different order.
 __device__ __forceinline__ void repaint_cond(float* z, float* pocket, float* hist, const float* __restrict__ known,
                                              const float* __restrict__ com_pocket0, const float* __restrict__ fixed,
                                              const float* __restrict__ noise1, const float* __restrict__ noise2,
-                                             const float* coef, const JointSpan& sp, int A, int R, float (*red)[4]) {
+                                             const float* coef, const JointSpan& sp, int A, int R, float (*red)[4],
+                                             float* hist2 = nullptr) {
   const int g = blockIdx.x, l0 = sp.l0, l1 = sp.l1, p0 = sp.p0, p1 = sp.p1;
   const int D = 3 + A, DR = 3 + R;
   const float alpha_s = coef[0], sigma_s = coef[1], alpha_ts = coef[2], sigma_ts = coef[3];
@@ -505,18 +506,20 @@ __device__ __forceinline__ void repaint_cond(float* z, float* pocket, float* his
     __syncthreads();
     sub_rows3(z, l0, l1, D, com2);
   }
-  // the pocket coordinates (and the history with them) move by -comk + dx, then by -com2
-  if (hist) {
+  // the pocket coordinates (and the histories with them) move by -comk + dx, then by -com2
+  auto move = [&](float* h) {
     for (int i = l0 + threadIdx.x; i < l1; i += blockDim.x) {
       const size_t r = (size_t)i * D;
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        float h = (hist[r + c] - comk[c]) + dx[c];
-        if (noise2) h -= com2[c];
-        hist[r + c] = h;
+        float x = (h[r + c] - comk[c]) + dx[c];
+        if (noise2) x -= com2[c];
+        h[r + c] = x;
       }
     }
-  }
+  };
+  if (hist) move(hist);
+  if (hist2) move(hist2);
   for (int idx = p0 * DR + threadIdx.x; idx < p1 * DR; idx += blockDim.x) {
     const int c = idx % DR;
     if (c < 3) {
@@ -596,14 +599,15 @@ __global__ void __launch_bounds__(128) ddpm_joint_update_kernel(float* z_lig, fl
 //   z       = z_known * fixed + z_unknown * (1 - fixed)                                       (:774-775)
 //   if nx3: z = alpha_ts z + sigma_ts eps3 (eps3.x COM-free), joint COM of z.x removed        (sample_p_zt_given_zs, :479-501, :790-807)
 // coef = (alpha_s, sigma_s, alpha_{t|s}, sigma_{t|s}).  The blend keeps the frame of the unknown part; the 2M history (h_lig,
-// h_poc, or null) moves with z through the jump back's COM removal.
+// h_poc, or null) and the second 3M history (h2_lig, h2_poc, or null) move with z through the jump back's COM removal.
 __device__ __forceinline__ void repaint_joint(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
                                               const float* __restrict__ x0_lig, const float* __restrict__ x0_poc,
                                               const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
                                               const float* __restrict__ nx1, const float* __restrict__ nhl1,
                                               const float* __restrict__ nhp1, const float* __restrict__ nx3,
                                               const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* coef,
-                                              const JointSpan& sp, int NL, int A, int R, float (*red)[4]) {
+                                              const JointSpan& sp, int NL, int A, int R, float (*red)[4],
+                                              float* h2_lig = nullptr, float* h2_poc = nullptr) {
   const int D = 3 + A, DR = 3 + R;
   const float alpha_s = coef[0], sigma_s = coef[1], alpha_ts = coef[2], sigma_ts = coef[3];
   float n1[3];
@@ -667,6 +671,7 @@ __device__ __forceinline__ void repaint_joint(float* z_lig, float* z_poc, float*
     sub_rows3(z_lig, sp.l0, sp.l1, D, m);
     sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
     if (h_lig) { sub_rows3(h_lig, sp.l0, sp.l1, D, m); sub_rows3(h_poc, sp.p0, sp.p1, DR, m); }
+    if (h2_lig) { sub_rows3(h2_lig, sp.l0, sp.l1, D, m); sub_rows3(h2_poc, sp.p0, sp.p1, DR, m); }
   }
 }
 
@@ -822,6 +827,91 @@ __global__ void __launch_bounds__(128) ddpm_multistep_inpaint_kernel(
                             n3, nhl3, nhp3, k, sp, NL, A, R, commit, red);
   else
     multistep_repaint_cond(z_lig, z_poc, h_lig, eps_lig, known_lig, com_pocket0, fix_lig, n1, n3, k, sp, A, R, commit, red);
+}
+
+// ---- DPM-Solver++(3M) step and RePaint round, both models (the contract is in include/diffsbdd_b200.h) --------------------
+// k = (sigma_s/sigma_t, 1/alpha_t, sigma_t, k0, k1, k2).  One element: x0 = (z - sigma_t eps) * inv_alpha_t ;
+// z' = c0 z + k0 x0 + k1 m1 + k2 m2, with m1 read only when k1 != 0 and m2 only when k2 != 0.  commit: m2 <- m1 (x0 when
+// k1 == 0, so that m1 is still not read) and m1 <- x0.  Writes z' in place; returns z'.
+__device__ __forceinline__ float multistep3_elem(float* z, float* h1, float* h2, const float* __restrict__ eps, size_t idx,
+                                                 const float* k, int commit) {
+  const float x0 = (z[idx] - k[2] * eps[idx]) * k[1];
+  float v = k[0] * z[idx] + k[3] * x0;
+  float m1 = x0;
+  if (k[4] != 0.f) { m1 = h1[idx]; v += k[4] * m1; }
+  if (k[5] != 0.f) v += k[5] * h2[idx];
+  z[idx] = v;
+  if (commit) { h2[idx] = m1; h1[idx] = x0; }
+  return v;
+}
+
+// The 3M step of one graph with its COM removal: the ligand COM of z'.x (joint == 0), removed from z', the pocket coordinates
+// and both ligand histories; or the ligand + pocket COM (joint != 0), removed from z' and both histories of both parts.
+__device__ __forceinline__ void multistep3_step(float* z_lig, float* z_poc, float* h1_lig, float* h1_poc, float* h2_lig,
+                                                float* h2_poc, const float* __restrict__ eps_lig,
+                                                const float* __restrict__ eps_poc, const float* k, const JointSpan& sp, int A,
+                                                int R, int joint, int commit, float (*red)[4]) {
+  const int D = 3 + A, DR = 3 + R;
+  float s[3] = {0.f, 0.f, 0.f};
+  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
+    const float v = multistep3_elem(z_lig, h1_lig, h2_lig, eps_lig, (size_t)idx, k, commit);
+    const int c = idx % D;
+    if (c < 3) s[c] += v;
+  }
+  if (joint) {
+    for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
+      const float v = multistep3_elem(z_poc, h1_poc, h2_poc, eps_poc, (size_t)idx, k, commit);
+      const int c = idx % DR;
+      if (c < 3) s[c] += v;
+    }
+  }
+  block_sum(s, 3, red);
+  const float cnt = joint ? sp.n : ((sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f);
+  const float m[3] = {s[0] / cnt, s[1] / cnt, s[2] / cnt};
+  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(h1_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(h2_lig, sp.l0, sp.l1, D, m);
+  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
+  if (joint) { sub_rows3(h1_poc, sp.p0, sp.p1, DR, m); sub_rows3(h2_poc, sp.p0, sp.p1, DR, m); }
+  __syncthreads();                      // z', the pocket and the histories are complete
+}
+
+// dsb_ddpm_multistep3_update: one block per graph.
+__global__ void __launch_bounds__(128) ddpm_multistep3_kernel(float* z_lig, float* z_poc, float* h1_lig, float* h1_poc,
+                                                               float* h2_lig, float* h2_poc, const float* __restrict__ eps_lig,
+                                                               const float* __restrict__ eps_poc, const float* __restrict__ coef,
+                                                               const int64_t* __restrict__ mask_atoms,
+                                                               const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R,
+                                                               int joint) {
+  __shared__ float red[9][4];
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
+  float k[6];
+#pragma unroll
+  for (int i = 0; i < 6; ++i) k[i] = coef[blockIdx.x * 6 + i];
+  multistep3_step(z_lig, z_poc, h1_lig, h1_poc, h2_lig, h2_poc, eps_lig, eps_poc, k, sp, A, R, joint, 1, red);
+}
+
+// dsb_ddpm_multistep3_inpaint_update: one block per graph; coef row g = the 3M row (6) then the RePaint row (4).  The 3M step,
+// then the model's RePaint iteration with both histories, which take every translation it applies.
+__global__ void __launch_bounds__(128) ddpm_multistep3_inpaint_kernel(
+    float* z_lig, float* z_poc, float* h1_lig, float* h1_poc, float* h2_lig, float* h2_poc, const float* __restrict__ eps_lig,
+    const float* __restrict__ eps_poc, const float* __restrict__ known_lig, const float* __restrict__ known_poc,
+    const float* __restrict__ com_pocket0, const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
+    const float* __restrict__ n1, const float* __restrict__ nhl1, const float* __restrict__ nhp1, const float* __restrict__ n3,
+    const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* __restrict__ coef,
+    const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R, int joint,
+    int commit) {
+  __shared__ float red[9][4];
+  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
+  float k[10];
+#pragma unroll
+  for (int i = 0; i < 10; ++i) k[i] = coef[blockIdx.x * 10 + i];
+  multistep3_step(z_lig, z_poc, h1_lig, h1_poc, h2_lig, h2_poc, eps_lig, eps_poc, k, sp, A, R, joint, commit, red);
+  if (joint)
+    repaint_joint(z_lig, z_poc, h1_lig, h1_poc, known_lig, known_poc, fix_lig, fix_poc, n1, nhl1, nhp1, n3, nhl3, nhp3, k + 6,
+                  sp, NL, A, R, red, h2_lig, h2_poc);
+  else
+    repaint_cond(z_lig, z_poc, h1_lig, known_lig, com_pocket0, fix_lig, n1, n3, k + 6, sp, A, R, red, h2_lig);
 }
 
 // ---- seeded per-graph random numbers (dsb_seeded_normal; the contract is in include/diffsbdd_b200.h) -------------------
@@ -1391,6 +1481,48 @@ int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist
       z_lig, z_pocket, hist_lig, hist_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0, lig_fixed, pocket_fixed,
       noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket, coef, mask_atoms,
       mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_multistep3_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
+                               float* hist2_pocket, const float* eps_lig, const float* eps_pocket, const float* coef,
+                               const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues,
+                               int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!z_lig || !hist_lig || !hist2_lig || !eps_lig || !coef || !mask_atoms || (n_residues > 0 && (!z_pocket || !mask_residues)) ||
+      (joint && n_residues > 0 && (!hist_pocket || !hist2_pocket || !eps_pocket))) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  ddpm_multistep3_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig,
+                                                                              hist2_pocket, eps_lig, eps_pocket, coef, mask_atoms,
+                                                                              mask_residues, (int)n_atoms, (int)n_residues, atom_nf,
+                                                                              residue_nf, joint != 0);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int dsb_ddpm_multistep3_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
+                                       float* hist2_pocket, const float* eps_lig, const float* eps_pocket, const float* known_lig,
+                                       const float* known_pocket, const float* com_pocket0, const float* lig_fixed,
+                                       const float* pocket_fixed, const float* noise_known, const float* noise_known_h_lig,
+                                       const float* noise_known_h_pocket, const float* renoise, const float* renoise_h_lig,
+                                       const float* renoise_h_pocket, const float* coef, const int64_t* mask_atoms,
+                                       const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                                       int32_t atom_nf, int32_t residue_nf, int32_t joint, int32_t commit, void* stream) {
+  if (n_graphs <= 0) return 0;
+  if (!z_lig || !hist_lig || !hist2_lig || !eps_lig || !known_lig || !lig_fixed || !noise_known || !coef || !mask_atoms ||
+      (n_residues > 0 && (!z_pocket || !mask_residues)) ||
+      (joint ? (!noise_known_h_lig || (renoise && !renoise_h_lig) ||
+                (n_residues > 0 && (!hist_pocket || !hist2_pocket || !eps_pocket || !known_pocket || !pocket_fixed ||
+                                    !noise_known_h_pocket || (renoise && !renoise_h_pocket))))
+             : !com_pocket0)) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  ddpm_multistep3_inpaint_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
+      z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig, hist2_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0,
+      lig_fixed, pocket_fixed, noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket,
+      coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
   DSB_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -117,7 +117,8 @@ def cosine_alphas2(timesteps: int, s: float = 0.008):
 
 
 # ---- few-step samplers (DESIGN §13) --------------------------------------------------------------------------------------
-SAMPLERS = ('ddpm', 'ddim', 'dpmpp_2m')
+SAMPLERS = ('ddpm', 'ddim', 'dpmpp_2m', 'dpmpp_3m')
+MULTISTEP = ('dpmpp_2m', 'dpmpp_3m')          # the samplers that keep x0_hat of earlier steps (DESIGN §13, §15)
 
 
 def check_sampler(sampler, eta):
@@ -130,8 +131,18 @@ def check_sampler(sampler, eta):
         raise ValueError(f"eta = {eta} needs sampler='ddim' ({sampler!r} is deterministic)")
 
 
+def _phi_remainder(h):
+    """(e^-h - 1 + h) / h^2 - 1/2 in float64 without the cancellation of the difference: below h = 1/4 its Taylor series
+    sum_{j >= 1} (-h)^j / (j + 2)!, summed by Horner to j = 16 (the remainder is below 1e-25 there)."""
+    series = torch.zeros_like(h)
+    for j in range(16, 0, -1):
+        series = (series + 1.0 / math.factorial(j + 2)) * (-h)
+    direct = (torch.expm1(-h) + h) / (h * h) - 0.5
+    return torch.where(h < 0.25, series, direct)
+
+
 def fast_coefficients(gamma_s, gamma_t, sampler, eta=0.0):
-    """float64 per-step coefficients of the 'ddim' and 'dpmpp_2m' steps from gamma at s and t ([N, 1] each, row k = step
+    """float64 per-step coefficients of the 'ddim', 'dpmpp_2m' and 'dpmpp_3m' steps from gamma at s and t ([N, 1] each, row k = step
     s = k, so that row k + 1 is the step run just before row k).  With alpha^2 = sigmoid(-gamma), sigma^2 = sigmoid(gamma):
 
     'ddim'     (alpha_{t|s}, alpha_s sigma_t / alpha_t - sqrt(sigma_s^2 - eta^2 st^2), eta st), st = sigma_{t|s} sigma_s / sigma_t:
@@ -139,7 +150,15 @@ def fast_coefficients(gamma_s, gamma_t, sampler, eta=0.0):
                eta^2 st^2) / (sigma_t / alpha_{t|s} + sqrt(sigma_s^2 - eta^2 st^2)), the same number without the cancellation
                of the difference, so that at eta = 1 it is the ancestral sigma^2_{t|s} / (alpha_{t|s} sigma_t) to rounding.
     'dpmpp_2m' (sigma_s / sigma_t, -alpha_s (e^-h - 1), 1 / alpha_t, sigma_t, w), h = lambda_s - lambda_t, lambda = -gamma / 2,
-               w = h / (2 h_prev) with h_prev the h of row k + 1, and w = 0 in the last row (the first step run)."""
+               w = h / (2 h_prev) with h_prev the h of row k + 1, and w = 0 in the last row (the first step run).
+    'dpmpp_3m' (sigma_s / sigma_t, 1 / alpha_t, sigma_t, k0, k1, k2): z_s = c0 z_t + k0 m0 + k1 m1 + k2 m2 with m0 = x0_hat of
+               this step and m1, m2 those of the two steps run before it (DESIGN §15).  The first step run (last row) is
+               DDIM at eta = 0 (k0 = -alpha_s phi1, phi1 = e^-h - 1), the second is 2M's second step (k0 = -alpha_s phi1
+               (1 + w), k1 = alpha_s phi1 w), every later one third order: with h1, h2 the h of rows k + 1, k + 2,
+               D1 = D1_0 + h1 / (h1 + h2) (D1_0 - D1_1), D2 = h (D1_0 - D1_1) / (h1 + h2), D1_0 = h (m0 - m1) / h1,
+               D1_1 = h (m1 - m2) / h2, z_s = c0 z_t - alpha_s phi1 m0 + alpha_s (phi1 / h + 1) D1 - alpha_s ((phi1 + h) / h^2
+               - 1/2) D2, collected per m.  phi1 / h + 1 = h (g + 1/2) and (phi1 + h) / h^2 - 1/2 = g come from
+               _phi_remainder, so no difference cancels at small h; every k is then a sum of same-signed terms."""
     gs, gt = gamma_s.detach().double(), gamma_t.detach().double()
     s2_s, s2_t = torch.sigmoid(gs), torch.sigmoid(gt)
     alpha_s, alpha_t = torch.sqrt(torch.sigmoid(-gs)), torch.sqrt(torch.sigmoid(-gt))
@@ -158,7 +177,31 @@ def fast_coefficients(gamma_s, gamma_t, sampler, eta=0.0):
         w = torch.zeros_like(h)
         w[:-1] = h[:-1] / (2.0 * h[1:])
         return torch.cat([sigma_s / sigma_t, -alpha_s * torch.expm1(-h), 1.0 / alpha_t, sigma_t, w], dim=1)
+    if sampler == 'dpmpp_3m':
+        h = 0.5 * (gt - gs)
+        c1 = -alpha_s * torch.expm1(-h)
+        g = _phi_remainder(h)
+        k = torch.zeros((h.shape[0], 3), dtype=h.dtype, device=h.device)
+        k[-1:, 0:1] = c1[-1:]                                       # first step run: order 1
+        if h.shape[0] >= 2:                                          # second: order 2, as 2M
+            w = h[-2:-1] / (2.0 * h[-1:])
+            k[-2:-1, 0:1], k[-2:-1, 1:2] = c1[-2:-1] * (1.0 + w), -c1[-2:-1] * w
+        if h.shape[0] >= 3:                                          # the rest: order 3
+            hh, h1, h2, a_s = h[:-2], h[1:-1], h[2:], alpha_s[:-2]
+            A, B = a_s * hh * (g[:-2] + 0.5), -a_s * g[:-2]          # alpha_s (phi1 / h + 1), -alpha_s ((phi1 + h) / h^2 - 1/2)
+            a0 = A * (1.0 + h1 / (h1 + h2)) + B * hh / (h1 + h2)     # the weights of D1_0 and D1_1
+            a1 = -A * h1 / (h1 + h2) - B * hh / (h1 + h2)
+            k[:-2] = torch.cat([c1[:-2] + a0 * hh / h1, -a0 * hh / h1 + a1 * hh / h2, -a1 * hh / h2], dim=1)
+        return torch.cat([sigma_s / sigma_t, 1.0 / alpha_t, sigma_t, k], dim=1)
     raise ValueError(sampler)
+
+
+def multistep3_update(z, eps, m1, m2, c):
+    """The 'dpmpp_3m' update of one part, rows of ``c`` per node (fast_coefficients): returns (z', x0_hat, m2'), where m2' =
+    m1, or x0_hat on the first step run (k1 = 0), is the next step's second history."""
+    x0 = (z - c[:, 2:3] * eps) * c[:, 1:2]
+    out = c[:, 0:1] * z + c[:, 3:4] * x0 + c[:, 4:5] * m1 + c[:, 5:6] * m2
+    return out, x0, torch.where(c[:, 4:5] != 0, m1, x0)
 
 
 class PredefinedNoiseSchedule(nn.Module):
@@ -517,7 +560,7 @@ class EnVariationalDiffusion(nn.Module):
         return t_arr.float().contiguous(), torch.cat(rev + inp, dim=1).float().contiguous()
 
     def _fast_tables(self, timesteps, sampler, eta, device, top=None):
-        """Per-step t and coefficients of the 'ddim' / 'dpmpp_2m' steps s = 0..timesteps-1 (t = s+1) for both engines:
+        """Per-step t and coefficients of the 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' steps s = 0..timesteps-1 (t = s+1) for both engines:
         fast_coefficients in float64 from the fp32 gamma values, cast to fp32, so that eager and graph steps use the same bits.
         ``top`` = (n, T): the grid ends at t* = n / T instead of 1 (diversify), t_k = k n / (timesteps T) in one rounding."""
         s_int = torch.arange(timesteps, device=device).view(-1, 1)
@@ -560,10 +603,13 @@ class EnVariationalDiffusion(nn.Module):
                           sampler=sampler)
                 for x in st['n_rev']:
                     x.zero_()
-                if sampler == 'dpmpp_2m':   # RePaint rounds: the 2M row and the RePaint row in one [n, 9] buffer
+                if sampler in MULTISTEP:   # RePaint rounds: the 2M / 3M row and the RePaint row in one [n, 9 | 10] buffer
                     st['hist'] = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket))
-                    st.update(ms_table=torch.cat((fast, coef_table[:, 3:]), 1).contiguous(),
-                              coef9=torch.zeros((n_samples, 9), device=device))
+                    if sampler == 'dpmpp_3m':
+                        st['hist2'] = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket))
+                    ms = torch.cat((fast, coef_table[:, 3:]), 1).contiguous()
+                    st['ms_table'] = ms
+                    st['coef9' if sampler == 'dpmpp_2m' else 'coef10'] = torch.zeros((n_samples, ms.shape[1]), device=device)
             self._joint_cache[key] = st
         if seeds is not None:
             st['seeds'].copy_(seeds)
@@ -572,12 +618,12 @@ class EnVariationalDiffusion(nn.Module):
 
     def _joint_step(self, st, kind):
         """kind: 'reverse' (sample: one joint reverse step, step -= 1) | 'inpaint' (noised known part + reverse step + blend,
-        step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1) | 'ddim' | 'dpmpp_2m'
-        (_joint_fast_captured_step).  The inpainting kinds of an engine built for a few-step sampler, and its 'inpaint_hold',
+        step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1) | 'ddim' | 'dpmpp_2m' |
+        'dpmpp_3m' (_joint_fast_captured_step).  The inpainting kinds of an engine built for a few-step sampler, and its 'inpaint_hold',
         are _joint_fast_inpaint_captured_step."""
         import ctypes as C
         from . import _native, seeded
-        if kind in ('ddim', 'dpmpp_2m'):
+        if kind in ('ddim',) + MULTISTEP:
             return self._joint_fast_captured_step(st, kind)
         if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
             return self._joint_fast_inpaint_captured_step(st, kind)
@@ -636,7 +682,7 @@ class EnVariationalDiffusion(nn.Module):
         st['zl'].copy_(z_lig); st['zp'].copy_(z_pocket); st['step'].fill_(first_s)
         if st['seeded']:
             st['u'].zero_()
-        for x in st.get('hist', ()):
+        for x in st.get('hist', ()) + st.get('hist2', ()):
             x.zero_()
 
     def _joint_graph(self, st, kind, z_lig, z_pocket, first_s):
@@ -686,9 +732,9 @@ class EnVariationalDiffusion(nn.Module):
         return st['zl'].clone(), st['zp'].clone()
 
     def _joint_fast_captured_step(self, st, kind):
-        """One 'ddim' or 'dpmpp_2m' step of the joint model over the static buffers of ``st`` (step -= 1): table row of
-        the step counter -> native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients (noise drawn only at eta > 0)
-        or dsb_ddpm_multistep_update."""
+        """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step of the joint model over the static buffers of ``st`` (step -= 1): table
+        row of the step counter -> native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients (noise drawn only at
+        eta > 0), dsb_ddpm_multistep_update or dsb_ddpm_multistep3_update."""
         import ctypes as C
         from . import _native, seeded
         dyn, lib = self.dynamics, _native.load()
@@ -718,18 +764,23 @@ class EnVariationalDiffusion(nn.Module):
                 _native.check(lib.dsb_ddpm_joint_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
                     ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            else:
+            elif kind == 'dpmpp_2m':
                 hl, hp = st['hist']
                 _native.check(lib.dsb_ddpm_multistep_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(st['coef_fast']), ptr(lm),
                     ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, stream))
+            else:
+                (hl, hp), (h2l, h2p) = st['hist'], st['hist2']
+                _native.check(lib.dsb_ddpm_multistep3_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(h2l), ptr(h2p), ptr(eps_l), ptr(eps_p),
+                    ptr(st['coef_fast']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, stream))
             st['step'].sub_(1)
         return run
 
     def _graphed_joint_fast_loop(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta,
                                  return_frames, out_lig, out_pocket):
-        """The whole 'ddim' / 'dpmpp_2m' reverse loop as ``timesteps`` replays of one captured step; frames are copied from
-        the static state between replays, so the history of the multistep sampler runs through them."""
+        """The whole 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' reverse loop as ``timesteps`` replays of one captured step; frames are
+        copied from the static state between replays, so the history of the multistep samplers runs through them."""
         dyn = self.dynamics
         st = self._joint_engine(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, 1, sampler, eta)
         s0 = timesteps - 1
@@ -748,9 +799,10 @@ class EnVariationalDiffusion(nn.Module):
         return st['zl'].clone(), st['zp'].clone()
 
     def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta, u=0):
-        """Eager 'ddim' / 'dpmpp_2m' step z_t -> z_s of the joint model (DESIGN §13); ``row`` [1, k]: the step's row of
-        _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step (2M only).
-        ``u``: the RePaint block of the seeded DDIM draw."""
+        """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s of the joint model (DESIGN §13, §15); ``row`` [1, k]: the
+        step's row of _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step
+        (2M), or per part the pair (m1, m2) of x0_hat of this step and of the one before it (3M).  ``u``: the RePaint block of
+        the seeded DDIM draw."""
         from . import seeded
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
@@ -764,6 +816,15 @@ class EnVariationalDiffusion(nn.Module):
                 mu_l, mu_p = self.sample_normal(mu_l, mu_p, c[:, 2:3], lig_mask, pocket_mask)
             zl, zp = self._project_joint_com(mu_l, mu_p, lig_mask, pocket_mask)
             return zl, zp, hl, hp
+        if sampler == 'dpmpp_3m':
+            zl, x0_l, m2_l = multistep3_update(zl, eps_l, *hl, cl)
+            zp, x0_p, m2_p = multistep3_update(zp, eps_p, *hp, cp)
+            mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lig_mask, pocket_mask)), dim=0,
+                                dim_size=t.shape[0])
+            for x, m in ((zl, lig_mask), (zp, pocket_mask), (x0_l, lig_mask), (x0_p, pocket_mask), (m2_l, lig_mask),
+                         (m2_p, pocket_mask)):
+                x[:, :nd] -= mean[m]
+            return zl, zp, (x0_l, m2_l), (x0_p, m2_p)
         x0_l = (zl - cl[:, 3:4] * eps_l) * cl[:, 2:3]
         x0_p = (zp - cp[:, 3:4] * eps_p) * cp[:, 2:3]
         zl = cl[:, 0:1] * zl + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0_l - cl[:, 4:5] * hl)
@@ -775,11 +836,11 @@ class EnVariationalDiffusion(nn.Module):
         return zl, zp, x0_l, x0_p
 
     def _joint_fast_inpaint_captured_step(self, st, kind):
-        """One RePaint iteration of an engine built for 'ddim' or 'dpmpp_2m' (DESIGN §14).  kind: 'inpaint' (blend; the
-        iteration commits its x0_hat as the 2M history; step -= 1) | 'inpaint_jump' (blend + jump back, no commit; step +=
+        """One RePaint iteration of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15).  kind: 'inpaint'
+        (blend; the iteration commits its x0_hat as the 2M / 3M history; step -= 1) | 'inpaint_jump' (blend + jump back, no commit; step +=
         jump_length - 1) | 'inpaint_hold' (blend, no commit, step -= 1: a frame is taken before an eager jump back).  DDIM:
         native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients -> dsb_ddpm_joint_inpaint_update.  2M: native
-        denoiser -> dsb_ddpm_multistep_inpaint_update."""
+        denoiser -> dsb_ddpm_multistep_inpaint_update.  3M: native denoiser -> dsb_ddpm_multistep3_inpaint_update."""
         import ctypes as C
         from . import _native, seeded
         dyn, lib = self.dynamics, _native.load()
@@ -788,6 +849,7 @@ class EnVariationalDiffusion(nn.Module):
         ptr = lambda x: x.data_ptr()
         roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
         ddim, jump = st['sampler'] == 'ddim', kind == 'inpaint_jump'
+        ms_key = 'coef9' if st['sampler'] == 'dpmpp_2m' else 'coef10'      # the 2M / 3M row + the RePaint row
 
         def draw(bufs, purpose):
             if st['seeded']:
@@ -808,7 +870,7 @@ class EnVariationalDiffusion(nn.Module):
                 st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
                 st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
             else:
-                st['coef9'].copy_(st['ms_table'].index_select(0, idx).expand(n, 9))
+                st[ms_key].copy_(st['ms_table'].index_select(0, idx).expand(n, st['ms_table'].shape[1]))
             eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
             if ddim and st['eta'] > 0:
                 draw(st['n_rev'], seeded.PURPOSE_REVERSE)
@@ -825,12 +887,18 @@ class EnVariationalDiffusion(nn.Module):
                     ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
                     *[ptr(x) for x in st['n_known']], *j, ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n,
                     self.atom_nf, self.residue_nf, stream))
-            else:
+            elif st['sampler'] == 'dpmpp_2m':
                 hl, hp = st['hist']
                 _native.check(lib.dsb_ddpm_multistep_inpaint_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(kn['xl']), ptr(kn['xp']), None,
-                    ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st['coef9']), ptr(lm), ptr(pm),
+                    ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st[ms_key]), ptr(lm), ptr(pm),
                     NL, NP, n, self.atom_nf, self.residue_nf, 1, int(kind == 'inpaint'), stream))
+            else:
+                (hl, hp), (h2l, h2p) = st['hist'], st['hist2']
+                _native.check(lib.dsb_ddpm_multistep3_inpaint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(h2l), ptr(h2p), ptr(eps_l), ptr(eps_p), ptr(kn['xl']),
+                    ptr(kn['xp']), None, ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st[ms_key]),
+                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, int(kind == 'inpaint'), stream))
             if jump:
                 st['step'].add_(st['jump'] - 1)
                 if st['seeded']:
@@ -845,8 +913,9 @@ class EnVariationalDiffusion(nn.Module):
         known part, the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row`` and t; 'ddim' / 'dpmpp_2m': the few-step
         step with ``row`` [1, k], the step's row of _fast_tables), the COM alignment and the blend.  ``hist``: () for
         'ddpm' and DDIM; for 2M (hist_lig, hist_pocket) = x0_hat committed by the last iteration of step s + 1, in the frame
-        of z.  The 2M COM removal moves it with z; the blend keeps the frame of the unknown part, so nothing else moves it;
-        ``commit``: this iteration's x0_hat becomes the history.  Returns (z_lig, z_pocket, hist)."""
+        of z; for 3M (m1_lig, m1_pocket, m2_lig, m2_pocket), m2 committed one step earlier.  The multistep COM removal moves
+        it with z; the blend keeps the frame of the unknown part, so nothing else moves it; ``commit``: this iteration's
+        x0_hat becomes the history (3M: m2 <- m1, m1 <- x0_hat).  Returns (z_lig, z_pocket, hist)."""
         from . import seeded
         nd = self.n_dims
         # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
@@ -857,6 +926,19 @@ class EnVariationalDiffusion(nn.Module):
             zu_lig, zu_pocket = self.sample_p_zs_given_zt(row, t, z_lig, z_pocket, lmask, pmask)
         elif sampler == 'ddim':
             zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, None, None, lmask, pmask, sampler, eta, i)
+        elif sampler == 'dpmpp_3m':
+            c = row.expand(t.shape[0], -1)
+            cl, cp = c[lmask], c[pmask]
+            m1l, m1p, m2l, m2p = (x.clone() for x in hist)
+            eps_l, eps_p = self.dynamics(z_lig, z_pocket, t, lmask, pmask)
+            zu_lig, x0_l, n2_l = multistep3_update(z_lig, eps_l, m1l, m2l, cl)
+            zu_pocket, x0_p, n2_p = multistep3_update(z_pocket, eps_p, m1p, m2p, cp)
+            mean = scatter_mean(torch.cat((zu_lig[:, :nd], zu_pocket[:, :nd])), torch.cat((lmask, pmask)), dim=0,
+                                dim_size=t.shape[0])
+            for x, m in ((zu_lig, lmask), (zu_pocket, pmask), (x0_l, lmask), (x0_p, pmask), (n2_l, lmask), (n2_p, pmask),
+                         (m1l, lmask), (m1p, pmask), (m2l, lmask), (m2p, pmask)):
+                x[:, :nd] -= mean[m]
+            hist = (x0_l, x0_p, n2_l, n2_p) if commit else (m1l, m1p, m2l, m2p)
         else:
             c = row.expand(t.shape[0], -1)
             cl, cp = c[lmask], c[pmask]
@@ -881,8 +963,8 @@ class EnVariationalDiffusion(nn.Module):
         return z_lig, z_pocket, hist
 
     def _joint_renoise(self, z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask):
-        """sample_p_zt_given_zs (the jump back, en_diffusion.py:790-807) with the 2M history ``hist`` (or ()) moved by the same
-        joint COM removal."""
+        """sample_p_zt_given_zs (the jump back, en_diffusion.py:790-807) with the multistep history ``hist`` (or ()) moved by
+        the same joint COM removal: (lig, pocket) pairs, as _joint_fast_inpaint_step keeps them."""
         if not hist:
             return (*self.sample_p_zt_given_zs(z_lig, z_pocket, lmask, pmask, gamma_t, gamma_s), ())
         nd = self.n_dims
@@ -890,7 +972,7 @@ class EnVariationalDiffusion(nn.Module):
         zl, zp = self.sample_normal(alpha_ts[lmask] * z_lig, alpha_ts[pmask] * z_pocket, sigma_ts, lmask, pmask)
         mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lmask, pmask)), dim=0)
         moved = []
-        for x, m in ((zl, lmask), (zp, pmask)) + tuple(zip(hist, (lmask, pmask))):
+        for x, m in ((zl, lmask), (zp, pmask)) + tuple(zip(hist, (lmask, pmask) * (len(hist) // 2))):
             x = x.clone()
             x[:, :nd] = x[:, :nd] - mean[m]
             moved.append(x)
@@ -902,8 +984,8 @@ class EnVariationalDiffusion(nn.Module):
                sampler='ddpm', eta=0.0):
         """en_diffusion.py:581-651: unconditional joint sampling of ligand and pocket.  ``seeds``: one int64 per sample
         (seeded.py); every draw then comes from the sample's own seed instead of torch's global generator.  ``sampler``:
-        'ddpm' (the reference's ancestral step), 'ddim' (with noise level ``eta`` in [0, 1]) or 'dpmpp_2m', on the same
-        ``timesteps`` grid (DESIGN §13)."""
+        'ddpm' (the reference's ancestral step), 'ddim' (with noise level ``eta`` in [0, 1]), 'dpmpp_2m' or 'dpmpp_3m', on
+        the same ``timesteps`` grid (DESIGN §13, §15)."""
         from . import seeded
         check_sampler(sampler, eta)
         seeds = seeded.as_seeds(seeds, n_samples, device)
@@ -930,7 +1012,7 @@ class EnVariationalDiffusion(nn.Module):
             self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         elif sampler != 'ddpm':
             t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
-            h_lig, h_pocket = torch.zeros_like(z_lig), torch.zeros_like(z_pocket)
+            h_lig, h_pocket = self._empty_history(z_lig, sampler), self._empty_history(z_pocket, sampler)
             for s in reversed(range(0, timesteps)):
                 z_lig, z_pocket, h_lig, h_pocket = self._joint_fast_step(
                     s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, z_pocket, h_lig, h_pocket, lig_mask, pocket_mask,
@@ -968,6 +1050,12 @@ class EnVariationalDiffusion(nn.Module):
         out_pocket[0] = torch.cat([x_pocket, h_pocket], dim=1)
         return out_lig.squeeze(0), out_pocket.squeeze(0), lig_mask, pocket_mask
 
+    @staticmethod
+    def _empty_history(x, sampler):
+        """The zero history of one part for the eager multistep steps: one tensor, or the pair (m1, m2) for 'dpmpp_3m'."""
+        h = torch.zeros_like(x)
+        return (h, h) if sampler == 'dpmpp_3m' else h
+
     # ---- RePaint-style inpainting with the joint model (en_diffusion.py:653-837) ---------------------------------
     @staticmethod
     def get_repaint_schedule(resamplings, jump_length, timesteps):
@@ -1004,13 +1092,13 @@ class EnVariationalDiffusion(nn.Module):
     def inpaint(self, ligand, pocket, lig_fixed, pocket_fixed, resamplings=1, jump_length=1, return_frames=1,
                 timesteps=None, seeds=None, sampler='ddpm', eta=0.0):
         """en_diffusion.py:677-837: sample the free nodes while the fixed ones follow q(z_s | x).  ``seeds``: as sample.
-        ``sampler`` / ``eta``: the reverse step of every RePaint iteration, as sample; 'dpmpp_2m' needs jump_length = 1
-        (DESIGN §14).  With every pocket node fixed this is how a joint model generates a ligand for a given pocket in few
+        ``sampler`` / ``eta``: the reverse step of every RePaint iteration, as sample; 'dpmpp_2m' and 'dpmpp_3m' need
+        jump_length = 1 (DESIGN §14, §15).  With every pocket node fixed this is how a joint model generates a ligand for a given pocket in few
         steps."""
         from . import seeded
         check_sampler(sampler, eta)
-        if sampler == 'dpmpp_2m' and jump_length > 1:
-            raise ValueError(f"sampler='dpmpp_2m' needs jump_length = 1 (got {jump_length}): its history has no rule for "
+        if sampler in MULTISTEP and jump_length > 1:
+            raise ValueError(f"sampler={sampler!r} needs jump_length = 1 (got {jump_length}): its history has no rule for "
                              f"jumps over several steps; use 'ddim'")
         seeds = seeded.as_seeds(seeds, len(ligand['size']), ligand['x'].device)
         with self._seeded(seeds, ligand['mask'], pocket['mask']):
@@ -1054,7 +1142,7 @@ class EnVariationalDiffusion(nn.Module):
         if self._joint_use_graph(z_lig.device):
             dyn = self.dynamics
             st = self._joint_engine(z_lig, z_pocket, lmask, pmask, n_samples, timesteps, jump_length, sampler, eta)
-            two_m = sampler == 'dpmpp_2m'
+            multistep = sampler in MULTISTEP
             if st['known'] is None:       # static buffers the captured RePaint iteration reads
                 st['known'] = dict(xl=torch.empty_like(xh0_lig), xp=torch.empty_like(xh0_pocket),
                                    fl=torch.empty(len(lmask), device=z_lig.device), fp=torch.empty(len(pmask), device=z_lig.device))
@@ -1064,18 +1152,18 @@ class EnVariationalDiffusion(nn.Module):
             try:
                 g_it = self._joint_graph(st, 'inpaint', z_lig, z_pocket, s)
                 g_jump = self._joint_graph(st, 'inpaint_jump', z_lig, z_pocket, s) if len(schedule) > 1 else None
-                # 2M: the frame-before-jump path replays an iteration that does not commit (captured here: a capture
+                # 2M / 3M: the frame-before-jump path replays an iteration that does not commit (captured here: a capture
                 # resets the static state)
-                g_hold = self._joint_graph(st, 'inpaint_hold', z_lig, z_pocket, s) if two_m and len(schedule) > 1 else None
+                g_hold = self._joint_graph(st, 'inpaint_hold', z_lig, z_pocket, s) if multistep and len(schedule) > 1 else None
                 self._joint_start(st, z_lig, z_pocket, s)
                 for i, n_denoise in enumerate(schedule):
                     for j in range(n_denoise):
                         jump = j == n_denoise - 1 and i < len(schedule) - 1
                         frame = (n_denoise > jump_length or i == len(schedule) - 1) and (s * return_frames) % timesteps == 0
                         # a frame is taken after the blend and BEFORE the jump back (en_diffusion.py:777-788): in that case the
-                        # jump runs as eager torch ops on the static state instead of inside the fused kernel (2M: after an
-                        # iteration that does not commit)
-                        if jump and frame and two_m:
+                        # jump runs as eager torch ops on the static state instead of inside the fused kernel (2M / 3M: after
+                        # an iteration that does not commit)
+                        if jump and frame and multistep:
                             g_hold.replay()
                         else:
                             (g_jump if (jump and not frame) else g_it).replay()
@@ -1089,7 +1177,7 @@ class EnVariationalDiffusion(nn.Module):
                                 t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
                                 g_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
                                 g_s = self.inflate_batch_array(self.gamma(s_arr), ligand['x'])
-                                hist = st.get('hist', ())
+                                hist = st.get('hist', ()) + st.get('hist2', ())
                                 zl, zp, moved = self._joint_renoise(st['zl'], st['zp'], hist, g_t, g_s, lmask, pmask)
                                 for x, y in zip(hist, moved):
                                     x.copy_(y)
@@ -1106,7 +1194,9 @@ class EnVariationalDiffusion(nn.Module):
         else:
             if sampler != 'ddpm':
                 t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
-            hist = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket)) if sampler == 'dpmpp_2m' else ()
+            hist = ()
+            if sampler in MULTISTEP:          # one (lig, pocket) pair per history: 2M keeps one, 3M two
+                hist = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket)) * (2 if sampler == 'dpmpp_3m' else 1)
             for i, n_denoise in enumerate(schedule):
                 for j in range(n_denoise):
                     jump = j == n_denoise - 1 and i < len(schedule) - 1

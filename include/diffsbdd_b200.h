@@ -307,6 +307,39 @@ int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist
                                       int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint,
                                       int32_t commit, void* stream);
 
+/* ---- DPM-Solver++(3M) step in data-prediction form (one launch, one block per graph; DESIGN §15), both models:
+ *   x0 = (z - sigma_t[g] eps_hat) * inv_alpha_t[g]
+ *   z' = c0[g] z + k0[g] x0 + k1[g] m1 + k2[g] m2 ; m1 = hist is read only when k1[g] != 0, m2 = hist2 only when k2[g] != 0
+ *   hist2' = m1 (x0 when k1[g] == 0) ; hist' = x0
+ * then the COM of z'.x is removed from z'.x, from the pocket coordinates and from hist'.x and hist2'.x, as in
+ * dsb_ddpm_multistep_update (joint == 0: the LIGAND COM, the pocket only shifted, hist_pocket, hist2_pocket and eps_pocket not
+ * used and may be NULL; joint != 0: ligand AND pocket updated, COM over ligand + pocket nodes).
+ * coef: device fp32 [n_graphs, 6] = (sigma_s/sigma_t, 1/alpha_t, sigma_t, k0, k1, k2): en_diffusion.fast_coefficients
+ * ('dpmpp_3m'), with k1 = k2 = 0 on the first step run and k2 = 0 on the second.  hist_* / hist2_* [rows, 3 + nf]: x0 of the
+ * previous step and of the one before it, in the current frame.  In place on z_*, hist_*, hist2_*.  Masks sorted; each graph's
+ * sums run in a fixed order without atomics, so the result repeats bit for bit and a graph's result does not depend on the rest
+ * of its batch. */
+int dsb_ddpm_multistep3_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
+                               float* hist2_pocket, const float* eps_lig, const float* eps_pocket, const float* coef,
+                               const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues,
+                               int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream);
+
+/* ---- RePaint round with the DPM-Solver++(3M) step (one launch, one block per graph; DESIGN §15), both models: as
+ * dsb_ddpm_multistep_inpaint_update with the 3M step of dsb_ddpm_multistep3_update in place of the 2M step.  Every translation
+ * the round applies to hist.x is applied to hist2.x too.  commit != 0: hist2 <- hist (x0 when k1 == 0) and hist <- x0 before
+ * those translations; commit == 0: both histories are only translated.
+ * coef: device fp32 [n_graphs, 10] = the 3M row (6) of dsb_ddpm_multistep3_update, then (alpha_s, sigma_s, alpha_{t|s},
+ * sigma_{t|s}) as the RePaint entries.  Pointers that a model does not use may be NULL as in
+ * dsb_ddpm_multistep_inpaint_update (hist2_pocket with hist_pocket). */
+int dsb_ddpm_multistep3_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
+                                       float* hist2_pocket, const float* eps_lig, const float* eps_pocket, const float* known_lig,
+                                       const float* known_pocket, const float* com_pocket0, const float* lig_fixed,
+                                       const float* pocket_fixed, const float* noise_known, const float* noise_known_h_lig,
+                                       const float* noise_known_h_pocket, const float* renoise, const float* renoise_h_lig,
+                                       const float* renoise_h_pocket, const float* coef, const int64_t* mask_atoms,
+                                       const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
+                                       int32_t atom_nf, int32_t residue_nf, int32_t joint, int32_t commit, void* stream);
+
 /* ---- evaluation-mode variational bound (validation / test NLL): what EnVariationalDiffusion.forward, ConditionalDDPM.forward
  * and SimpleConditionalDDPM.forward compute in eval mode besides the two denoiser calls and the per-graph scalar algebra.
  *
