@@ -155,6 +155,17 @@ def check(code: int) -> None:
         raise NativeError(f'libdiffsbdd_b200 error {code}: {msg}')
 
 
+def multistep_update(lib: C.CDLL, z, hist, eps, coef, masks, sizes, joint: int, stream, repaint=(), commit: int = 1) -> None:
+    """One DPM-Solver++ step, or with ``repaint`` one RePaint round, in place on device tensors: 2M with one history, 3M with
+    two (dsb_ddpm_multistep[3][_inpaint]_update).  ``z``, ``eps`` and each history, newest first: (ligand, pocket) pairs,
+    None where the conditional model has no pocket part; ``repaint``: the tensors known_lig .. renoise_h_pocket of the
+    RePaint entries (None where absent); ``sizes``: (n_atoms, n_residues, n_graphs, atom_nf, residue_nf)."""
+    ptr = lambda x: None if x is None else x.data_ptr()
+    name = 'dsb_ddpm_multistep%s%s_update' % ('3' if len(hist) == 2 else '', '_inpaint' if repaint else '')
+    bufs = (*z, *(x for h in hist for x in h), *eps, *repaint, coef, *masks)
+    check(getattr(lib, name)(*map(ptr, bufs), *sizes, joint, *((commit,) if repaint else ()), stream))
+
+
 def param_names(cfg: DsbConfig):
     lib = load()
     n = lib.dsb_param_count(C.byref(cfg))

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 
 from . import _native, seeded
 from .dynamics import EGNNDynamics
-from .en_diffusion import (MULTISTEP, EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, multistep3_update,
+from .en_diffusion import (MULTISTEP, EnVariationalDiffusion, check_sampler, follows_dynamics_determinism, multistep_update,
                            scatter_add, scatter_mean, num_nodes_to_batch_mask)
 
 
@@ -256,6 +256,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
             if key in st:
                 st[key].zero_()
 
+    @staticmethod
+    def _static_history(st):
+        """The multistep histories of the static state, newest first, as (ligand, no pocket part) pairs."""
+        return tuple((st[k], None) for k in ('hist', 'hist2') if k in st)
+
     def _graph(self, st, kind, z_lig, xh_pocket, first_s):
         """Captured CUDA graph of ``kind`` (captured on first use; capture leaves the static state as it found it)."""
         g = st['graphs'].get(kind)
@@ -309,8 +314,8 @@ class ConditionalDDPM(EnVariationalDiffusion):
 
     def _fast_captured_step(self, st, kind):
         """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step over the static buffers of ``st`` (step -= 1): table row of the step
-        counter -> native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0),
-        dsb_ddpm_multistep_update or dsb_ddpm_multistep3_update."""
+        counter -> native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0), or the
+        2M / 3M step (_native.multistep_update)."""
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
@@ -334,16 +339,9 @@ class ConditionalDDPM(EnVariationalDiffusion):
                     st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef_fast'].data_ptr(), lm.data_ptr(),
                     pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, st['z'].data_ptr(),
                     st['pocket'].data_ptr(), stream))
-            elif kind == 'dpmpp_2m':
-                _native.check(lib.dsb_ddpm_multistep_update(
-                    st['z'].data_ptr(), st['pocket'].data_ptr(), st['hist'].data_ptr(), None, eps.data_ptr(), None,
-                    st['coef_fast'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, 0,
-                    stream))
             else:
-                _native.check(lib.dsb_ddpm_multistep3_update(
-                    st['z'].data_ptr(), st['pocket'].data_ptr(), st['hist'].data_ptr(), None, st['hist2'].data_ptr(), None,
-                    eps.data_ptr(), None, st['coef_fast'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf,
-                    self.residue_nf, 0, stream))
+                _native.multistep_update(lib, (st['z'], st['pocket']), self._static_history(st), (eps, None), st['coef_fast'],
+                                         (lm, pm), (NL, NP, n, self.atom_nf, self.residue_nf), 0, stream)
             st['step'].sub_(1)
         return run
 
@@ -370,11 +368,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
         dyn.check_status()
         return st['z'].clone(), st['pocket'].clone()
 
-    def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta, u=0):
+    def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta, u=0, commit=True):
         """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s (DESIGN §13, §15); ``row`` [1, k]: the step's row of
-        _fast_tables.  Returns (z_lig, xh_pocket, hist); the history is x0_hat of this step (2M), or the pair (m1, m2) of x0_hat
-        of this step and of the one before it (3M), in the frame of the returned z.  ``u``: the resampling round of the seeded
-        DDIM draw (RePaint)."""
+        _fast_tables; ``hist``: the history (_empty_history).  Returns (z_lig, xh_pocket, hist): with ``commit`` the history
+        multistep_update writes, else the one given; either way moved by the step's ligand-COM removal, so that it stays in
+        the pocket's frame.  ``u``: the resampling round of the seeded DDIM draw (RePaint)."""
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
         cl = c[lig_mask]
@@ -389,31 +387,24 @@ class ConditionalDDPM(EnVariationalDiffusion):
                 mu[:, :nd], xh_pocket[:, :nd] = self.remove_mean_batch(mu[:, :nd], xh_pocket[:, :nd], lig_mask, pocket_mask)
                 z_lig = mu
             return z_lig, xh_pocket, hist
-        if sampler == 'dpmpp_3m':
-            # the ligand COM leaves z, the pocket and both histories together
-            NP, NL = xh_pocket.shape[0], z_lig.shape[0]
-            z_lig, x0, m2 = multistep3_update(z_lig, eps, *hist, cl)
-            xh_pocket = xh_pocket.clone()
-            z_lig[:, :nd], moved = self.remove_mean_batch(z_lig[:, :nd], torch.cat((xh_pocket[:, :nd], x0[:, :nd], m2[:, :nd])),
-                                                          lig_mask, torch.cat((pocket_mask, lig_mask, lig_mask)))
-            xh_pocket[:, :nd], x0[:, :nd], m2[:, :nd] = moved[:NP], moved[NP:NP + NL], moved[NP + NL:]
-            return z_lig, xh_pocket, (x0, m2)
-        x0 = (z_lig - cl[:, 3:4] * eps) * cl[:, 2:3]
-        z_lig = cl[:, 0:1] * z_lig + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0 - cl[:, 4:5] * hist)
-        # the ligand COM leaves z, the pocket and the history together (one mean, subtracted from both)
-        NP = xh_pocket.shape[0]
+        z_lig, new = multistep_update(z_lig, eps, hist, cl)
+        hist = new if commit else tuple(h.clone() for h in hist)
+        # the ligand COM leaves z, the pocket and the history together (one mean, subtracted from all)
+        NP, NL = xh_pocket.shape[0], z_lig.shape[0]
         xh_pocket = xh_pocket.clone()
-        z_lig[:, :nd], moved = self.remove_mean_batch(z_lig[:, :nd], torch.cat((xh_pocket[:, :nd], x0[:, :nd])), lig_mask,
-                                                      torch.cat((pocket_mask, lig_mask)))
-        xh_pocket[:, :nd], x0[:, :nd] = moved[:NP], moved[NP:]
-        return z_lig, xh_pocket, x0
+        z_lig[:, :nd], moved = self.remove_mean_batch(
+            z_lig[:, :nd], torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hist)), lig_mask,
+            torch.cat((pocket_mask,) + (lig_mask,) * len(hist)))
+        xh_pocket[:, :nd] = moved[:NP]
+        for k, h in enumerate(hist):
+            h[:, :nd] = moved[NP + k * NL:NP + (k + 1) * NL]
+        return z_lig, xh_pocket, hist
 
     def _fast_inpaint_captured_step(self, st, kind):
         """One RePaint round of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15); kind as _captured_step
         ('inpaint_renoise': re-noised, the round does not commit; 'inpaint_last': the last round of the step, which commits
         its x0_hat as the 2M / 3M history).  DDIM: native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients ->
-        dsb_ddpm_inpaint_update.  2M: native denoiser -> dsb_ddpm_multistep_inpaint_update.  3M: native denoiser ->
-        dsb_ddpm_multistep3_inpaint_update."""
+        dsb_ddpm_inpaint_update.  2M / 3M: native denoiser -> the fused RePaint round (_native.multistep_update)."""
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
@@ -447,24 +438,20 @@ class ConditionalDDPM(EnVariationalDiffusion):
             if renoise:
                 draw(st['noise2'], seeded.PURPOSE_RENOISE)
             ip = st['inpaint']
-            n2 = ptr(st['noise2']) if renoise else None
             if ddim:
+                n2 = ptr(st['noise2']) if renoise else None
                 _native.check(lib.dsb_ddpm_ligand_update(
                     ptr(st['z']), ptr(eps), ptr(st['noise']), ptr(st['coef_fast']), ptr(lm), ptr(pm), ptr(st['pocket']), NL, NP,
                     n, self.atom_nf, self.residue_nf, ptr(st['z']), ptr(st['pocket']), stream))
                 _native.check(lib.dsb_ddpm_inpaint_update(
                     ptr(st['z']), ptr(st['pocket']), ptr(ip['known']), ptr(ip['com0']), ptr(ip['fixed']), ptr(st['noise1']), n2,
                     ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            elif st['sampler'] == 'dpmpp_2m':
-                _native.check(lib.dsb_ddpm_multistep_inpaint_update(
-                    ptr(st['z']), ptr(st['pocket']), ptr(st['hist']), None, ptr(eps), None, ptr(ip['known']), None,
-                    ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None, ptr(st[ms_key]),
-                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 0, int(not renoise), stream))
             else:
-                _native.check(lib.dsb_ddpm_multistep3_inpaint_update(
-                    ptr(st['z']), ptr(st['pocket']), ptr(st['hist']), None, ptr(st['hist2']), None, ptr(eps), None,
-                    ptr(ip['known']), None, ptr(ip['com0']), ptr(ip['fixed']), None, ptr(st['noise1']), None, None, n2, None, None,
-                    ptr(st[ms_key]), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 0, int(not renoise), stream))
+                _native.multistep_update(
+                    lib, (st['z'], st['pocket']), self._static_history(st), (eps, None), st[ms_key], (lm, pm),
+                    (NL, NP, n, self.atom_nf, self.residue_nf), 0, stream,
+                    (ip['known'], None, ip['com0'], ip['fixed'], None, st['noise1'], None, None,
+                     st['noise2'] if renoise else None, None, None), int(not renoise))
             if renoise:
                 if st['seeded']:
                     st['u'].add_(1)
@@ -478,35 +465,25 @@ class ConditionalDDPM(EnVariationalDiffusion):
                            lig_fixed, lmask, pmask, sampler, eta, last):
         """Eager RePaint round (s, u) of _inpaint (DESIGN §14): the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row``
         and t; 'ddim' / 'dpmpp_2m' / 'dpmpp_3m': the few-step step with ``row`` [1, k], the step's row of _fast_tables), then
-        the known part, the COM alignment, the blend and, unless ``last``, the re-noising.  2M: ``hist`` is x0_hat committed
-        by the last round of step s + 1, kept in the pocket's frame: every translation of the pocket coordinates moves it
-        too, and the last round of step s commits its own x0_hat.  3M: ``hist`` is the pair (m1, m2) under the same rule; the
-        commit is m2 <- m1, m1 <- x0_hat.  Returns (z_lig, xh_pocket, hist)."""
+        the known part, the COM alignment, the blend and, unless ``last``, the re-noising.  ``hist`` (_empty_history) is the
+        history committed by the last round of step s + 1, kept in the pocket's frame: every translation of the pocket
+        coordinates moves it too, and the last round of step s commits its own (multistep_update); 'ddpm' and DDIM leave it
+        as it is.  Returns (z_lig, xh_pocket, hist)."""
         nd, NL, NP = self.n_dims, z_lig.shape[0], xh_pocket.shape[0]
         fixed_rows = lig_fixed.bool().view(-1)
+        hists = ()          # the multistep history, moved by the step
         if sampler == 'ddpm':
             self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
             z_unknown, xh_pocket = self.sample_p_zs_given_zt(row, t, z_lig, xh_pocket, lmask, pmask)
         elif sampler == 'ddim':
-            z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u)
-        if sampler not in MULTISTEP:
-            # only the x columns of the pocket are ever translated
-            frame, fmask = xh_pocket[:, :nd], pmask
+            z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, (), lmask, pmask, sampler, eta, u)
         else:
-            c = row.expand(t.shape[0], -1)[lmask]
-            eps, _ = self.dynamics(z_lig, xh_pocket, t, lmask, pmask)
-            if sampler == 'dpmpp_2m':
-                x0 = (z_lig - c[:, 3:4] * eps) * c[:, 2:3]
-                z_unknown = c[:, 0:1] * z_lig + c[:, 1:2] * ((1 + c[:, 4:5]) * x0 - c[:, 4:5] * hist)
-                hists = (hist,)
-            else:           # (m1, m2, and the m2 a commit would write)
-                z_unknown, x0, m2_next = multistep3_update(z_lig, eps, *hist, c)
-                hists = hist + (m2_next,)
-            # frame: the rows that every pocket translation moves (pocket, histories, x0_hat), under the pocket's graph index
-            fmask = torch.cat((pmask,) + (lmask,) * (len(hists) + 1))
-            z_unknown[:, :nd], frame = self.remove_mean_batch(
-                z_unknown[:, :nd], torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hists) + (x0[:, :nd],)), lmask,
-                fmask)
+            z_unknown, xh_pocket, hists = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u,
+                                                          last)
+        # frame: the rows that every pocket translation moves (the pocket's x columns and the history), under the pocket's
+        # graph index
+        frame = torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hists))
+        fmask = torch.cat((pmask,) + (lmask,) * len(hists))
 
         # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
         com_pocket = scatter_mean(frame[:NP], pmask, dim=0)
@@ -524,14 +501,8 @@ class ConditionalDDPM(EnVariationalDiffusion):
             self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_RENOISE)
             z_lig, frame = self.sample_p_zt_given_zs(z_lig, frame, lmask, fmask, gamma_t, gamma_s)
         xh_pocket = torch.cat((frame[:NP], xh_pocket[:, nd:]), dim=1)
-        if sampler == 'dpmpp_2m':
-            keep = x0 if last else hist
-            rows = frame[NP + NL:] if last else frame[NP:NP + NL]
-            hist = torch.cat((rows, keep[:, nd:]), dim=1)
-        elif sampler == 'dpmpp_3m':
-            keep = (x0, m2_next) if last else hist
-            rows = (frame[NP + 3 * NL:], frame[NP + 2 * NL:NP + 3 * NL]) if last else (frame[NP:NP + NL], frame[NP + NL:NP + 2 * NL])
-            hist = tuple(torch.cat((r, k[:, nd:]), dim=1) for r, k in zip(rows, keep))
+        if hists:
+            hist = tuple(torch.cat((frame[NP + k * NL:NP + (k + 1) * NL], h[:, nd:]), dim=1) for k, h in enumerate(hists))
         return z_lig, xh_pocket, hist
 
     def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,

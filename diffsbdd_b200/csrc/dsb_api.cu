@@ -688,179 +688,53 @@ __global__ void __launch_bounds__(128) ddpm_joint_inpaint_kernel(
 }
 
 
-// ---- DPM-Solver++(2M) step of both models (the contract is in include/diffsbdd_b200.h) ---------------------------------
-// One element of the step: x0 = (z - sigma_t eps) * inv_alpha_t ; D = (1 + w) x0 - w hist (x0 alone when w = 0, so the
-// history is not read on a first step) ; z' = c0 z + c1 D.  Writes z' and x0 in place; returns z'.
-__device__ __forceinline__ float multistep_elem(float* z, float* hist, const float* __restrict__ eps, size_t idx, float c0,
-                                                float c1, float inv_alpha, float sigma, float w) {
-  const float x0 = (z[idx] - sigma * eps[idx]) * inv_alpha;
-  const float d = w != 0.f ? (1.f + w) * x0 - w * hist[idx] : x0;
-  const float v = c0 * z[idx] + c1 * d;
-  z[idx] = v;
-  hist[idx] = x0;
-  return v;
+// ---- DPM-Solver++(2M) and (3M) steps and RePaint rounds, both models (the contracts are in include/diffsbdd_b200.h) ------
+// One element of the step, for ORDER 2 or 3.  Writes z' in place and, when `commit`, the histories; returns z'.
+//   2M: k = (c0, c1, 1/alpha_t, sigma_t, w).  x0 = (z - sigma_t eps) * inv_alpha_t ; D = (1 + w) x0 - w m1 (x0 when w = 0,
+//       so the history is not read on a first step) ; z' = c0 z + c1 D, with one product rounded and the other fused into
+//       the sum: c0 z in the plain step, c1 D in the RePaint round (the roundings these kernels have always had, pinned
+//       with intrinsics so that their outputs stay bit for bit).  commit: m1 <- x0.
+//   3M: k = (c0, 1/alpha_t, sigma_t, k0, k1, k2).  z' = c0 z + k0 x0 + k1 m1 + k2 m2, with m1 read only when k1 != 0 and m2
+//       only when k2 != 0.  commit: m2 <- m1 (x0 when k1 == 0, so that m1 is still not read) and m1 <- x0.
+template <int ORDER, bool REPAINT>
+__device__ __forceinline__ float multistep_elem(float* z, float* h1, float* h2, const float* __restrict__ eps, size_t idx,
+                                                const float* k, int commit) {
+  if constexpr (ORDER == 2) {
+    const float x0 = (z[idx] - k[3] * eps[idx]) * k[2];
+    const float d = k[4] != 0.f ? (1.f + k[4]) * x0 - k[4] * h1[idx] : x0;
+    const float v = REPAINT ? __fmaf_rn(k[0], z[idx], __fmul_rn(k[1], d)) : __fmaf_rn(k[1], d, __fmul_rn(k[0], z[idx]));
+    z[idx] = v;
+    if (commit) h1[idx] = x0;
+    return v;
+  } else {
+    const float x0 = (z[idx] - k[2] * eps[idx]) * k[1];
+    float v = k[0] * z[idx] + k[3] * x0;
+    float m1 = x0;
+    if (k[4] != 0.f) { m1 = h1[idx]; v += k[4] * m1; }
+    if (k[5] != 0.f) v += k[5] * h2[idx];
+    z[idx] = v;
+    if (commit) { h2[idx] = m1; h1[idx] = x0; }
+    return v;
+  }
 }
 
-// One block per graph; the COM of z'.x (ligand only, or ligand + pocket when `joint`) is summed in a fixed order and
-// removed from z', from the pocket coordinates and from the history written by this step.
-__global__ void __launch_bounds__(128) ddpm_multistep_kernel(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
-                                                              const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
-                                                              const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms,
-                                                              const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R,
-                                                              int joint) {
-  const int g = blockIdx.x;
-  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, g);
+// The step of one graph with its COM removal: the ligand COM of z'.x (joint == 0), removed from z', the pocket coordinates
+// and the ligand histories; or the ligand + pocket COM (joint != 0), removed from z' and the histories of both parts.
+template <int ORDER, bool REPAINT>
+__device__ __forceinline__ void multistep_step(float* z_lig, float* z_poc, float* h1_lig, float* h1_poc, float* h2_lig,
+                                               float* h2_poc, const float* __restrict__ eps_lig,
+                                               const float* __restrict__ eps_poc, const float* k, const JointSpan& sp, int A,
+                                               int R, int joint, int commit, float (*red)[4]) {
   const int D = 3 + A, DR = 3 + R;
-  const float c0 = coef[g * 5 + 0], c1 = coef[g * 5 + 1], inv_alpha = coef[g * 5 + 2], sigma = coef[g * 5 + 3],
-              w = coef[g * 5 + 4];
-  __shared__ float red[9][4];
   float s[3] = {0.f, 0.f, 0.f};
   for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const float v = multistep_elem(z_lig, h_lig, eps_lig, (size_t)idx, c0, c1, inv_alpha, sigma, w);
+    const float v = multistep_elem<ORDER, REPAINT>(z_lig, h1_lig, h2_lig, eps_lig, (size_t)idx, k, commit);
     const int c = idx % D;
     if (c < 3) s[c] += v;
   }
   if (joint) {
     for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
-      const float v = multistep_elem(z_poc, h_poc, eps_poc, (size_t)idx, c0, c1, inv_alpha, sigma, w);
-      const int c = idx % DR;
-      if (c < 3) s[c] += v;
-    }
-  }
-  block_sum(s, 3, red);
-  const float cnt = joint ? sp.n : ((sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f);
-  const float m[3] = {s[0] / cnt, s[1] / cnt, s[2] / cnt};
-  __syncthreads();
-  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
-  sub_rows3(h_lig, sp.l0, sp.l1, D, m);
-  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
-  if (joint) sub_rows3(h_poc, sp.p0, sp.p1, DR, m);
-}
-
-
-// ---- RePaint round with the DPM-Solver++(2M) step, both models (the contract is in include/diffsbdd_b200.h) -----------
-// The 2M part of one element: z' = c0 z + c1 D with D from x0 = (z - sigma_t eps) * inv_alpha_t and the history; x0 replaces
-// the history only when the round commits.  Returns z'.
-__device__ __forceinline__ float multistep_repaint_elem(float* z, float* hist, const float* __restrict__ eps, size_t idx,
-                                                        const float* k, int commit) {
-  const float x0 = (z[idx] - k[3] * eps[idx]) * k[2];
-  const float d = k[4] != 0.f ? (1.f + k[4]) * x0 - k[4] * hist[idx] : x0;
-  const float v = k[0] * z[idx] + k[1] * d;
-  z[idx] = v;
-  if (commit) hist[idx] = x0;
-  return v;
-}
-
-// Conditional model: the 2M step with its ligand-COM removal, which moves the pocket and the history too, then repaint_cond
-// with the history.
-__device__ __forceinline__ void multistep_repaint_cond(float* z, float* pocket, float* hist, const float* __restrict__ eps,
-                                                       const float* __restrict__ known, const float* __restrict__ com_pocket0,
-                                                       const float* __restrict__ fixed, const float* __restrict__ noise1,
-                                                       const float* __restrict__ noise2, const float* k, const JointSpan& sp,
-                                                       int A, int R, int commit, float (*red)[4]) {
-  const int D = 3 + A, DR = 3 + R;
-  const float nl = (sp.l1 - sp.l0) > 0 ? (float)(sp.l1 - sp.l0) : 1.f;
-  float v[3] = {0.f, 0.f, 0.f};
-  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const float o = multistep_repaint_elem(z, hist, eps, (size_t)idx, k, commit);
-    const int c = idx % D;
-    if (c < 3) v[c] += o;
-  }
-  block_sum(v, 3, red);
-  const float m[3] = {v[0] / nl, v[1] / nl, v[2] / nl};
-  sub_rows3(z, sp.l0, sp.l1, D, m);
-  sub_rows3(hist, sp.l0, sp.l1, D, m);
-  sub_rows3(pocket, sp.p0, sp.p1, DR, m);
-  __syncthreads();                      // z = z_unknown and the moved pocket are complete
-  repaint_cond(z, pocket, hist, known, com_pocket0, fixed, noise1, noise2, k + 5, sp, A, R, red);
-}
-
-// Joint model: the 2M step of ligand and pocket with the joint COM removal, which moves the history too, then repaint_joint
-// with the history.
-__device__ __forceinline__ void multistep_repaint_joint(float* z_lig, float* z_poc, float* h_lig, float* h_poc,
-                                                        const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
-                                                        const float* __restrict__ x0_lig, const float* __restrict__ x0_poc,
-                                                        const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
-                                                        const float* __restrict__ nx1, const float* __restrict__ nhl1,
-                                                        const float* __restrict__ nhp1, const float* __restrict__ nx3,
-                                                        const float* __restrict__ nhl3, const float* __restrict__ nhp3,
-                                                        const float* k, const JointSpan& sp, int NL, int A, int R, int commit,
-                                                        float (*red)[4]) {
-  const int D = 3 + A, DR = 3 + R;
-  float v[3] = {0.f, 0.f, 0.f};
-  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const float o = multistep_repaint_elem(z_lig, h_lig, eps_lig, (size_t)idx, k, commit);
-    const int c = idx % D;
-    if (c < 3) v[c] += o;
-  }
-  for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
-    const float o = multistep_repaint_elem(z_poc, h_poc, eps_poc, (size_t)idx, k, commit);
-    const int c = idx % DR;
-    if (c < 3) v[c] += o;
-  }
-  block_sum(v, 3, red);
-  const float m[3] = {v[0] / sp.n, v[1] / sp.n, v[2] / sp.n};
-  sub_rows3(z_lig, sp.l0, sp.l1, D, m);
-  sub_rows3(h_lig, sp.l0, sp.l1, D, m);
-  sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
-  sub_rows3(h_poc, sp.p0, sp.p1, DR, m);
-  __syncthreads();                      // z = the unknown part, complete
-  repaint_joint(z_lig, z_poc, h_lig, h_poc, x0_lig, x0_poc, fix_lig, fix_poc, nx1, nhl1, nhp1, nx3, nhl3, nhp3, k + 5, sp, NL,
-                A, R, red);
-}
-
-// One block per graph; coef row g = the 2M row (5) then the RePaint row (4).
-__global__ void __launch_bounds__(128) ddpm_multistep_inpaint_kernel(
-    float* z_lig, float* z_poc, float* h_lig, float* h_poc, const float* __restrict__ eps_lig, const float* __restrict__ eps_poc,
-    const float* __restrict__ known_lig, const float* __restrict__ known_poc, const float* __restrict__ com_pocket0,
-    const float* __restrict__ fix_lig, const float* __restrict__ fix_poc, const float* __restrict__ n1, const float* __restrict__ nhl1,
-    const float* __restrict__ nhp1, const float* __restrict__ n3, const float* __restrict__ nhl3, const float* __restrict__ nhp3,
-    const float* __restrict__ coef, const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP,
-    int A, int R, int joint, int commit) {
-  __shared__ float red[9][4];
-  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
-  float k[9];
-#pragma unroll
-  for (int i = 0; i < 9; ++i) k[i] = coef[blockIdx.x * 9 + i];
-  if (joint)
-    multistep_repaint_joint(z_lig, z_poc, h_lig, h_poc, eps_lig, eps_poc, known_lig, known_poc, fix_lig, fix_poc, n1, nhl1, nhp1,
-                            n3, nhl3, nhp3, k, sp, NL, A, R, commit, red);
-  else
-    multistep_repaint_cond(z_lig, z_poc, h_lig, eps_lig, known_lig, com_pocket0, fix_lig, n1, n3, k, sp, A, R, commit, red);
-}
-
-// ---- DPM-Solver++(3M) step and RePaint round, both models (the contract is in include/diffsbdd_b200.h) --------------------
-// k = (sigma_s/sigma_t, 1/alpha_t, sigma_t, k0, k1, k2).  One element: x0 = (z - sigma_t eps) * inv_alpha_t ;
-// z' = c0 z + k0 x0 + k1 m1 + k2 m2, with m1 read only when k1 != 0 and m2 only when k2 != 0.  commit: m2 <- m1 (x0 when
-// k1 == 0, so that m1 is still not read) and m1 <- x0.  Writes z' in place; returns z'.
-__device__ __forceinline__ float multistep3_elem(float* z, float* h1, float* h2, const float* __restrict__ eps, size_t idx,
-                                                 const float* k, int commit) {
-  const float x0 = (z[idx] - k[2] * eps[idx]) * k[1];
-  float v = k[0] * z[idx] + k[3] * x0;
-  float m1 = x0;
-  if (k[4] != 0.f) { m1 = h1[idx]; v += k[4] * m1; }
-  if (k[5] != 0.f) v += k[5] * h2[idx];
-  z[idx] = v;
-  if (commit) { h2[idx] = m1; h1[idx] = x0; }
-  return v;
-}
-
-// The 3M step of one graph with its COM removal: the ligand COM of z'.x (joint == 0), removed from z', the pocket coordinates
-// and both ligand histories; or the ligand + pocket COM (joint != 0), removed from z' and both histories of both parts.
-__device__ __forceinline__ void multistep3_step(float* z_lig, float* z_poc, float* h1_lig, float* h1_poc, float* h2_lig,
-                                                float* h2_poc, const float* __restrict__ eps_lig,
-                                                const float* __restrict__ eps_poc, const float* k, const JointSpan& sp, int A,
-                                                int R, int joint, int commit, float (*red)[4]) {
-  const int D = 3 + A, DR = 3 + R;
-  float s[3] = {0.f, 0.f, 0.f};
-  for (int idx = sp.l0 * D + threadIdx.x; idx < sp.l1 * D; idx += blockDim.x) {
-    const float v = multistep3_elem(z_lig, h1_lig, h2_lig, eps_lig, (size_t)idx, k, commit);
-    const int c = idx % D;
-    if (c < 3) s[c] += v;
-  }
-  if (joint) {
-    for (int idx = sp.p0 * DR + threadIdx.x; idx < sp.p1 * DR; idx += blockDim.x) {
-      const float v = multistep3_elem(z_poc, h1_poc, h2_poc, eps_poc, (size_t)idx, k, commit);
+      const float v = multistep_elem<ORDER, REPAINT>(z_poc, h1_poc, h2_poc, eps_poc, (size_t)idx, k, commit);
       const int c = idx % DR;
       if (c < 3) s[c] += v;
     }
@@ -870,30 +744,20 @@ __device__ __forceinline__ void multistep3_step(float* z_lig, float* z_poc, floa
   const float m[3] = {s[0] / cnt, s[1] / cnt, s[2] / cnt};
   sub_rows3(z_lig, sp.l0, sp.l1, D, m);
   sub_rows3(h1_lig, sp.l0, sp.l1, D, m);
-  sub_rows3(h2_lig, sp.l0, sp.l1, D, m);
+  if (ORDER == 3) sub_rows3(h2_lig, sp.l0, sp.l1, D, m);
   sub_rows3(z_poc, sp.p0, sp.p1, DR, m);
-  if (joint) { sub_rows3(h1_poc, sp.p0, sp.p1, DR, m); sub_rows3(h2_poc, sp.p0, sp.p1, DR, m); }
+  if (joint) {
+    sub_rows3(h1_poc, sp.p0, sp.p1, DR, m);
+    if (ORDER == 3) sub_rows3(h2_poc, sp.p0, sp.p1, DR, m);
+  }
   __syncthreads();                      // z', the pocket and the histories are complete
 }
 
-// dsb_ddpm_multistep3_update: one block per graph.
-__global__ void __launch_bounds__(128) ddpm_multistep3_kernel(float* z_lig, float* z_poc, float* h1_lig, float* h1_poc,
-                                                               float* h2_lig, float* h2_poc, const float* __restrict__ eps_lig,
-                                                               const float* __restrict__ eps_poc, const float* __restrict__ coef,
-                                                               const int64_t* __restrict__ mask_atoms,
-                                                               const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R,
-                                                               int joint) {
-  __shared__ float red[9][4];
-  const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
-  float k[6];
-#pragma unroll
-  for (int i = 0; i < 6; ++i) k[i] = coef[blockIdx.x * 6 + i];
-  multistep3_step(z_lig, z_poc, h1_lig, h1_poc, h2_lig, h2_poc, eps_lig, eps_poc, k, sp, A, R, joint, 1, red);
-}
-
-// dsb_ddpm_multistep3_inpaint_update: one block per graph; coef row g = the 3M row (6) then the RePaint row (4).  The 3M step,
-// then the model's RePaint iteration with both histories, which take every translation it applies.
-__global__ void __launch_bounds__(128) ddpm_multistep3_inpaint_kernel(
+// One block per graph; coef row g = the step's row (5 for 2M, 6 for 3M), then with REPAINT the RePaint row (4).  With REPAINT
+// the step commits only when `commit`, and the model's RePaint iteration follows, moving the histories with every
+// translation it applies.
+template <int ORDER, bool REPAINT>
+__global__ void __launch_bounds__(128) ddpm_multistep_kernel(
     float* z_lig, float* z_poc, float* h1_lig, float* h1_poc, float* h2_lig, float* h2_poc, const float* __restrict__ eps_lig,
     const float* __restrict__ eps_poc, const float* __restrict__ known_lig, const float* __restrict__ known_poc,
     const float* __restrict__ com_pocket0, const float* __restrict__ fix_lig, const float* __restrict__ fix_poc,
@@ -901,17 +765,21 @@ __global__ void __launch_bounds__(128) ddpm_multistep3_inpaint_kernel(
     const float* __restrict__ nhl3, const float* __restrict__ nhp3, const float* __restrict__ coef,
     const int64_t* __restrict__ mask_atoms, const int64_t* __restrict__ mask_res, int NL, int NP, int A, int R, int joint,
     int commit) {
+  constexpr int NS = ORDER == 2 ? 5 : 6, NK = NS + (REPAINT ? 4 : 0);
   __shared__ float red[9][4];
   const JointSpan sp = joint_span(mask_atoms, mask_res, NL, NP, blockIdx.x);
-  float k[10];
+  float k[NK];
 #pragma unroll
-  for (int i = 0; i < 10; ++i) k[i] = coef[blockIdx.x * 10 + i];
-  multistep3_step(z_lig, z_poc, h1_lig, h1_poc, h2_lig, h2_poc, eps_lig, eps_poc, k, sp, A, R, joint, commit, red);
-  if (joint)
-    repaint_joint(z_lig, z_poc, h1_lig, h1_poc, known_lig, known_poc, fix_lig, fix_poc, n1, nhl1, nhp1, n3, nhl3, nhp3, k + 6,
-                  sp, NL, A, R, red, h2_lig, h2_poc);
-  else
-    repaint_cond(z_lig, z_poc, h1_lig, known_lig, com_pocket0, fix_lig, n1, n3, k + 6, sp, A, R, red, h2_lig);
+  for (int i = 0; i < NK; ++i) k[i] = coef[blockIdx.x * NK + i];
+  multistep_step<ORDER, REPAINT>(z_lig, z_poc, h1_lig, h1_poc, h2_lig, h2_poc, eps_lig, eps_poc, k, sp, A, R, joint,
+                                 REPAINT ? commit : 1, red);
+  if constexpr (REPAINT) {
+    if (joint)
+      repaint_joint(z_lig, z_poc, h1_lig, h1_poc, known_lig, known_poc, fix_lig, fix_poc, n1, nhl1, nhp1, n3, nhl3, nhp3, k + NS,
+                    sp, NL, A, R, red, h2_lig, h2_poc);
+    else
+      repaint_cond(z_lig, z_poc, h1_lig, known_lig, com_pocket0, fix_lig, n1, n3, k + NS, sp, A, R, red, h2_lig);
+  }
 }
 
 // ---- seeded per-graph random numbers (dsb_seeded_normal; the contract is in include/diffsbdd_b200.h) -------------------
@@ -1443,21 +1311,45 @@ int dsb_ddpm_joint_update(float* z_lig, float* z_pocket, const float* eps_lig, c
   return 0;
 }
 
+// The four multistep entry points: `order` 2 or 3, the plain step or (`repaint`) the RePaint round.  hist2_* are read only by
+// 3M; known_* to renoise_* only by the RePaint round.
+static int multistep_launch(int order, bool repaint, float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket,
+                            float* hist2_lig, float* hist2_pocket, const float* eps_lig, const float* eps_pocket,
+                            const float* known_lig, const float* known_pocket, const float* com_pocket0, const float* lig_fixed,
+                            const float* pocket_fixed, const float* noise_known, const float* noise_known_h_lig,
+                            const float* noise_known_h_pocket, const float* renoise, const float* renoise_h_lig,
+                            const float* renoise_h_pocket, const float* coef, const int64_t* mask_atoms,
+                            const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs, int32_t atom_nf,
+                            int32_t residue_nf, int32_t joint, int32_t commit, void* stream) {
+  if (n_graphs <= 0) return 0;
+  const bool m3 = order == 3;
+  if (!z_lig || !hist_lig || (m3 && !hist2_lig) || !eps_lig || !coef || !mask_atoms ||
+      (n_residues > 0 && (!z_pocket || !mask_residues)) ||
+      (joint && n_residues > 0 && (!hist_pocket || (m3 && !hist2_pocket) || !eps_pocket)) ||
+      (repaint && (!known_lig || !lig_fixed || !noise_known ||
+                   (joint ? (!noise_known_h_lig || (renoise && !renoise_h_lig) ||
+                             (n_residues > 0 && (!known_pocket || !pocket_fixed || !noise_known_h_pocket ||
+                                                 (renoise && !renoise_h_pocket))))
+                          : !com_pocket0)))) {
+    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
+  }
+  auto kernel = m3 ? (repaint ? ddpm_multistep_kernel<3, true> : ddpm_multistep_kernel<3, false>)
+                   : (repaint ? ddpm_multistep_kernel<2, true> : ddpm_multistep_kernel<2, false>);
+  kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
+      z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig, hist2_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0,
+      lig_fixed, pocket_fixed, noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket,
+      coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
+  DSB_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 int dsb_ddpm_multistep_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
                               const float* eps_pocket, const float* coef, const int64_t* mask_atoms,
                               const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
                               int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream) {
-  if (n_graphs <= 0) return 0;
-  if (!z_lig || !hist_lig || !eps_lig || !coef || !mask_atoms || (n_residues > 0 && (!z_pocket || !mask_residues)) ||
-      (joint && n_residues > 0 && (!hist_pocket || !eps_pocket))) {
-    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
-  }
-  ddpm_multistep_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(z_lig, z_pocket, hist_lig, hist_pocket, eps_lig,
-                                                                             eps_pocket, coef, mask_atoms, mask_residues,
-                                                                             (int)n_atoms, (int)n_residues, atom_nf, residue_nf,
-                                                                             joint != 0);
-  DSB_CUDA_OK(cudaGetLastError());
-  return 0;
+  return multistep_launch(2, false, z_lig, z_pocket, hist_lig, hist_pocket, nullptr, nullptr, eps_lig, eps_pocket, nullptr,
+                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, coef,
+                          mask_atoms, mask_residues, n_atoms, n_residues, n_graphs, atom_nf, residue_nf, joint, 1, stream);
 }
 
 int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, const float* eps_lig,
@@ -1468,38 +1360,19 @@ int dsb_ddpm_multistep_inpaint_update(float* z_lig, float* z_pocket, float* hist
                                       const float* coef, const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms,
                                       int64_t n_residues, int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint,
                                       int32_t commit, void* stream) {
-  if (n_graphs <= 0) return 0;
-  if (!z_lig || !hist_lig || !eps_lig || !known_lig || !lig_fixed || !noise_known || !coef || !mask_atoms ||
-      (n_residues > 0 && (!z_pocket || !mask_residues)) ||
-      (joint ? (!noise_known_h_lig || (renoise && !renoise_h_lig) ||
-                (n_residues > 0 && (!hist_pocket || !eps_pocket || !known_pocket || !pocket_fixed || !noise_known_h_pocket ||
-                                    (renoise && !renoise_h_pocket))))
-             : !com_pocket0)) {
-    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
-  }
-  ddpm_multistep_inpaint_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
-      z_lig, z_pocket, hist_lig, hist_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0, lig_fixed, pocket_fixed,
-      noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket, coef, mask_atoms,
-      mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
-  DSB_CUDA_OK(cudaGetLastError());
-  return 0;
+  return multistep_launch(2, true, z_lig, z_pocket, hist_lig, hist_pocket, nullptr, nullptr, eps_lig, eps_pocket, known_lig,
+                          known_pocket, com_pocket0, lig_fixed, pocket_fixed, noise_known, noise_known_h_lig,
+                          noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket, coef, mask_atoms, mask_residues,
+                          n_atoms, n_residues, n_graphs, atom_nf, residue_nf, joint, commit, stream);
 }
 
 int dsb_ddpm_multistep3_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
                                float* hist2_pocket, const float* eps_lig, const float* eps_pocket, const float* coef,
                                const int64_t* mask_atoms, const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues,
                                int64_t n_graphs, int32_t atom_nf, int32_t residue_nf, int32_t joint, void* stream) {
-  if (n_graphs <= 0) return 0;
-  if (!z_lig || !hist_lig || !hist2_lig || !eps_lig || !coef || !mask_atoms || (n_residues > 0 && (!z_pocket || !mask_residues)) ||
-      (joint && n_residues > 0 && (!hist_pocket || !hist2_pocket || !eps_pocket))) {
-    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
-  }
-  ddpm_multistep3_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig,
-                                                                              hist2_pocket, eps_lig, eps_pocket, coef, mask_atoms,
-                                                                              mask_residues, (int)n_atoms, (int)n_residues, atom_nf,
-                                                                              residue_nf, joint != 0);
-  DSB_CUDA_OK(cudaGetLastError());
-  return 0;
+  return multistep_launch(3, false, z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig, hist2_pocket, eps_lig, eps_pocket,
+                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, coef,
+                          mask_atoms, mask_residues, n_atoms, n_residues, n_graphs, atom_nf, residue_nf, joint, 1, stream);
 }
 
 int dsb_ddpm_multistep3_inpaint_update(float* z_lig, float* z_pocket, float* hist_lig, float* hist_pocket, float* hist2_lig,
@@ -1510,21 +1383,10 @@ int dsb_ddpm_multistep3_inpaint_update(float* z_lig, float* z_pocket, float* his
                                        const float* renoise_h_pocket, const float* coef, const int64_t* mask_atoms,
                                        const int64_t* mask_residues, int64_t n_atoms, int64_t n_residues, int64_t n_graphs,
                                        int32_t atom_nf, int32_t residue_nf, int32_t joint, int32_t commit, void* stream) {
-  if (n_graphs <= 0) return 0;
-  if (!z_lig || !hist_lig || !hist2_lig || !eps_lig || !known_lig || !lig_fixed || !noise_known || !coef || !mask_atoms ||
-      (n_residues > 0 && (!z_pocket || !mask_residues)) ||
-      (joint ? (!noise_known_h_lig || (renoise && !renoise_h_lig) ||
-                (n_residues > 0 && (!hist_pocket || !hist2_pocket || !eps_pocket || !known_pocket || !pocket_fixed ||
-                                    !noise_known_h_pocket || (renoise && !renoise_h_pocket))))
-             : !com_pocket0)) {
-    set_error("null pointer"); return DSB_ERR_INVALID_ARGUMENT;
-  }
-  ddpm_multistep3_inpaint_kernel<<<(unsigned)n_graphs, 128, 0, (cudaStream_t)stream>>>(
-      z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig, hist2_pocket, eps_lig, eps_pocket, known_lig, known_pocket, com_pocket0,
-      lig_fixed, pocket_fixed, noise_known, noise_known_h_lig, noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket,
-      coef, mask_atoms, mask_residues, (int)n_atoms, (int)n_residues, atom_nf, residue_nf, joint != 0, commit != 0);
-  DSB_CUDA_OK(cudaGetLastError());
-  return 0;
+  return multistep_launch(3, true, z_lig, z_pocket, hist_lig, hist_pocket, hist2_lig, hist2_pocket, eps_lig, eps_pocket,
+                          known_lig, known_pocket, com_pocket0, lig_fixed, pocket_fixed, noise_known, noise_known_h_lig,
+                          noise_known_h_pocket, renoise, renoise_h_lig, renoise_h_pocket, coef, mask_atoms, mask_residues,
+                          n_atoms, n_residues, n_graphs, atom_nf, residue_nf, joint, commit, stream);
 }
 
 int dsb_ddpm_joint_inpaint_update(float* z_lig, float* z_pocket, const float* xh0_lig, const float* xh0_pocket,

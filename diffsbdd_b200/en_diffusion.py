@@ -196,12 +196,17 @@ def fast_coefficients(gamma_s, gamma_t, sampler, eta=0.0):
     raise ValueError(sampler)
 
 
-def multistep3_update(z, eps, m1, m2, c):
-    """The 'dpmpp_3m' update of one part, rows of ``c`` per node (fast_coefficients): returns (z', x0_hat, m2'), where m2' =
-    m1, or x0_hat on the first step run (k1 = 0), is the next step's second history."""
+def multistep_update(z, eps, hist, c):
+    """The 'dpmpp_2m' / 'dpmpp_3m' update of one part, rows of ``c`` per node (fast_coefficients), before its COM removal.
+    ``hist``: the x0_hat of the steps run before, newest first: (m1,) for 2M, (m1, m2) for 3M.  Returns (z', the history a
+    commit writes): (x0_hat,) for 2M; (x0_hat, m2') for 3M, where m2' = m1, or x0_hat on the first step run (k1 = 0)."""
+    if len(hist) == 1:
+        x0 = (z - c[:, 3:4] * eps) * c[:, 2:3]
+        return c[:, 0:1] * z + c[:, 1:2] * ((1 + c[:, 4:5]) * x0 - c[:, 4:5] * hist[0]), (x0,)
+    m1, m2 = hist
     x0 = (z - c[:, 2:3] * eps) * c[:, 1:2]
     out = c[:, 0:1] * z + c[:, 3:4] * x0 + c[:, 4:5] * m1 + c[:, 5:6] * m2
-    return out, x0, torch.where(c[:, 4:5] != 0, m1, x0)
+    return out, (x0, torch.where(c[:, 4:5] != 0, m1, x0))
 
 
 class PredefinedNoiseSchedule(nn.Module):
@@ -685,6 +690,11 @@ class EnVariationalDiffusion(nn.Module):
         for x in st.get('hist', ()) + st.get('hist2', ()):
             x.zero_()
 
+    @staticmethod
+    def _joint_static_history(st):
+        """The multistep histories of the static state, newest first, as (lig, pocket) pairs: () | (hist,) | (hist, hist2)."""
+        return tuple(st[k] for k in ('hist', 'hist2') if k in st)
+
     def _joint_graph(self, st, kind, z_lig, z_pocket, first_s):
         g = st['graphs'].get(kind)
         if g is not None:
@@ -734,7 +744,7 @@ class EnVariationalDiffusion(nn.Module):
     def _joint_fast_captured_step(self, st, kind):
         """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step of the joint model over the static buffers of ``st`` (step -= 1): table
         row of the step counter -> native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients (noise drawn only at
-        eta > 0), dsb_ddpm_multistep_update or dsb_ddpm_multistep3_update."""
+        eta > 0), or the 2M / 3M step (_native.multistep_update)."""
         import ctypes as C
         from . import _native, seeded
         dyn, lib = self.dynamics, _native.load()
@@ -764,16 +774,9 @@ class EnVariationalDiffusion(nn.Module):
                 _native.check(lib.dsb_ddpm_joint_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
                     ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            elif kind == 'dpmpp_2m':
-                hl, hp = st['hist']
-                _native.check(lib.dsb_ddpm_multistep_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(st['coef_fast']), ptr(lm),
-                    ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, stream))
             else:
-                (hl, hp), (h2l, h2p) = st['hist'], st['hist2']
-                _native.check(lib.dsb_ddpm_multistep3_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(h2l), ptr(h2p), ptr(eps_l), ptr(eps_p),
-                    ptr(st['coef_fast']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, stream))
+                _native.multistep_update(lib, (st['zl'], st['zp']), self._joint_static_history(st), (eps_l, eps_p),
+                                         st['coef_fast'], (lm, pm), (NL, NP, n, self.atom_nf, self.residue_nf), 1, stream)
             st['step'].sub_(1)
         return run
 
@@ -798,11 +801,12 @@ class EnVariationalDiffusion(nn.Module):
         dyn.check_status()
         return st['zl'].clone(), st['zp'].clone()
 
-    def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta, u=0):
+    def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta, u=0, commit=True):
         """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s of the joint model (DESIGN §13, §15); ``row`` [1, k]: the
-        step's row of _fast_tables.  Returns (z_lig, z_pocket, hist_lig, hist_pocket); the history is x0_hat of this step
-        (2M), or per part the pair (m1, m2) of x0_hat of this step and of the one before it (3M).  ``u``: the RePaint block of
-        the seeded DDIM draw."""
+        step's row of _fast_tables.  ``hl``, ``hp``: the history of each part (_empty_history).  Returns (z_lig, z_pocket,
+        hist_lig, hist_pocket): with ``commit`` the history multistep_update writes, else the one given; either way moved
+        by the step's joint COM removal, so that it stays in the frame of z.  ``u``: the RePaint block of the seeded DDIM
+        draw."""
         from . import seeded
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
@@ -816,31 +820,24 @@ class EnVariationalDiffusion(nn.Module):
                 mu_l, mu_p = self.sample_normal(mu_l, mu_p, c[:, 2:3], lig_mask, pocket_mask)
             zl, zp = self._project_joint_com(mu_l, mu_p, lig_mask, pocket_mask)
             return zl, zp, hl, hp
-        if sampler == 'dpmpp_3m':
-            zl, x0_l, m2_l = multistep3_update(zl, eps_l, *hl, cl)
-            zp, x0_p, m2_p = multistep3_update(zp, eps_p, *hp, cp)
-            mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lig_mask, pocket_mask)), dim=0,
-                                dim_size=t.shape[0])
-            for x, m in ((zl, lig_mask), (zp, pocket_mask), (x0_l, lig_mask), (x0_p, pocket_mask), (m2_l, lig_mask),
-                         (m2_p, pocket_mask)):
-                x[:, :nd] -= mean[m]
-            return zl, zp, (x0_l, m2_l), (x0_p, m2_p)
-        x0_l = (zl - cl[:, 3:4] * eps_l) * cl[:, 2:3]
-        x0_p = (zp - cp[:, 3:4] * eps_p) * cp[:, 2:3]
-        zl = cl[:, 0:1] * zl + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0_l - cl[:, 4:5] * hl)
-        zp = cp[:, 0:1] * zp + cp[:, 1:2] * ((1 + cp[:, 4:5]) * x0_p - cp[:, 4:5] * hp)
+        zl, new_l = multistep_update(zl, eps_l, hl, cl)
+        zp, new_p = multistep_update(zp, eps_p, hp, cp)
+        if commit:
+            hl, hp = new_l, new_p
+        else:
+            hl, hp = tuple(x.clone() for x in hl), tuple(x.clone() for x in hp)
         mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lig_mask, pocket_mask)), dim=0,
                             dim_size=t.shape[0])
-        for x, m in ((zl, lig_mask), (zp, pocket_mask), (x0_l, lig_mask), (x0_p, pocket_mask)):
+        for x, m in ((zl, lig_mask), (zp, pocket_mask), *((x, lig_mask) for x in hl), *((x, pocket_mask) for x in hp)):
             x[:, :nd] -= mean[m]
-        return zl, zp, x0_l, x0_p
+        return zl, zp, hl, hp
 
     def _joint_fast_inpaint_captured_step(self, st, kind):
         """One RePaint iteration of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15).  kind: 'inpaint'
         (blend; the iteration commits its x0_hat as the 2M / 3M history; step -= 1) | 'inpaint_jump' (blend + jump back, no commit; step +=
         jump_length - 1) | 'inpaint_hold' (blend, no commit, step -= 1: a frame is taken before an eager jump back).  DDIM:
-        native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients -> dsb_ddpm_joint_inpaint_update.  2M: native
-        denoiser -> dsb_ddpm_multistep_inpaint_update.  3M: native denoiser -> dsb_ddpm_multistep3_inpaint_update."""
+        native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients -> dsb_ddpm_joint_inpaint_update.  2M / 3M:
+        native denoiser -> the fused RePaint round (_native.multistep_update)."""
         import ctypes as C
         from . import _native, seeded
         dyn, lib = self.dynamics, _native.load()
@@ -877,8 +874,8 @@ class EnVariationalDiffusion(nn.Module):
             if jump:
                 draw(st['n_jump'], seeded.PURPOSE_RENOISE)
             kn = st['known']
-            j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
             if ddim:
+                j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
                 nx, nhl, nhp = st['n_rev']
                 _native.check(lib.dsb_ddpm_joint_update(
                     ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
@@ -887,18 +884,12 @@ class EnVariationalDiffusion(nn.Module):
                     ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
                     *[ptr(x) for x in st['n_known']], *j, ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n,
                     self.atom_nf, self.residue_nf, stream))
-            elif st['sampler'] == 'dpmpp_2m':
-                hl, hp = st['hist']
-                _native.check(lib.dsb_ddpm_multistep_inpaint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(eps_l), ptr(eps_p), ptr(kn['xl']), ptr(kn['xp']), None,
-                    ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st[ms_key]), ptr(lm), ptr(pm),
-                    NL, NP, n, self.atom_nf, self.residue_nf, 1, int(kind == 'inpaint'), stream))
             else:
-                (hl, hp), (h2l, h2p) = st['hist'], st['hist2']
-                _native.check(lib.dsb_ddpm_multistep3_inpaint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(hl), ptr(hp), ptr(h2l), ptr(h2p), ptr(eps_l), ptr(eps_p), ptr(kn['xl']),
-                    ptr(kn['xp']), None, ptr(kn['fl']), ptr(kn['fp']), *[ptr(x) for x in st['n_known']], *j, ptr(st[ms_key]),
-                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, 1, int(kind == 'inpaint'), stream))
+                _native.multistep_update(
+                    lib, (st['zl'], st['zp']), self._joint_static_history(st), (eps_l, eps_p), st[ms_key], (lm, pm),
+                    (NL, NP, n, self.atom_nf, self.residue_nf), 1, stream,
+                    (kn['xl'], kn['xp'], None, kn['fl'], kn['fp'], *st['n_known'], *(st['n_jump'] if jump else (None,) * 3)),
+                    int(kind == 'inpaint'))
             if jump:
                 st['step'].add_(st['jump'] - 1)
                 if st['seeded']:
@@ -912,10 +903,10 @@ class EnVariationalDiffusion(nn.Module):
         """Eager RePaint iteration (s, block i) of the joint inpaint (DESIGN §14), without the jump back (_joint_renoise): the
         known part, the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row`` and t; 'ddim' / 'dpmpp_2m': the few-step
         step with ``row`` [1, k], the step's row of _fast_tables), the COM alignment and the blend.  ``hist``: () for
-        'ddpm' and DDIM; for 2M (hist_lig, hist_pocket) = x0_hat committed by the last iteration of step s + 1, in the frame
-        of z; for 3M (m1_lig, m1_pocket, m2_lig, m2_pocket), m2 committed one step earlier.  The multistep COM removal moves
-        it with z; the blend keeps the frame of the unknown part, so nothing else moves it; ``commit``: this iteration's
-        x0_hat becomes the history (3M: m2 <- m1, m1 <- x0_hat).  Returns (z_lig, z_pocket, hist)."""
+        'ddpm' and DDIM; for the multistep samplers (hist_lig, hist_pocket) as _joint_fast_step takes them, committed by the
+        last iteration of step s + 1, in the frame of z.  The multistep COM removal moves it with z; the blend keeps the
+        frame of the unknown part, so nothing else moves it; ``commit``: this iteration writes the history
+        (multistep_update).  Returns (z_lig, z_pocket, hist)."""
         from . import seeded
         nd = self.n_dims
         # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
@@ -925,34 +916,11 @@ class EnVariationalDiffusion(nn.Module):
             self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_REVERSE)
             zu_lig, zu_pocket = self.sample_p_zs_given_zt(row, t, z_lig, z_pocket, lmask, pmask)
         elif sampler == 'ddim':
-            zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, None, None, lmask, pmask, sampler, eta, i)
-        elif sampler == 'dpmpp_3m':
-            c = row.expand(t.shape[0], -1)
-            cl, cp = c[lmask], c[pmask]
-            m1l, m1p, m2l, m2p = (x.clone() for x in hist)
-            eps_l, eps_p = self.dynamics(z_lig, z_pocket, t, lmask, pmask)
-            zu_lig, x0_l, n2_l = multistep3_update(z_lig, eps_l, m1l, m2l, cl)
-            zu_pocket, x0_p, n2_p = multistep3_update(z_pocket, eps_p, m1p, m2p, cp)
-            mean = scatter_mean(torch.cat((zu_lig[:, :nd], zu_pocket[:, :nd])), torch.cat((lmask, pmask)), dim=0,
-                                dim_size=t.shape[0])
-            for x, m in ((zu_lig, lmask), (zu_pocket, pmask), (x0_l, lmask), (x0_p, pmask), (n2_l, lmask), (n2_p, pmask),
-                         (m1l, lmask), (m1p, pmask), (m2l, lmask), (m2p, pmask)):
-                x[:, :nd] -= mean[m]
-            hist = (x0_l, x0_p, n2_l, n2_p) if commit else (m1l, m1p, m2l, m2p)
+            zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, (), (), lmask, pmask, sampler, eta, i)
         else:
-            c = row.expand(t.shape[0], -1)
-            cl, cp = c[lmask], c[pmask]
-            hl, hp = (x.clone() for x in hist)
-            eps_l, eps_p = self.dynamics(z_lig, z_pocket, t, lmask, pmask)
-            x0_l = (z_lig - cl[:, 3:4] * eps_l) * cl[:, 2:3]
-            x0_p = (z_pocket - cp[:, 3:4] * eps_p) * cp[:, 2:3]
-            zu_lig = cl[:, 0:1] * z_lig + cl[:, 1:2] * ((1 + cl[:, 4:5]) * x0_l - cl[:, 4:5] * hl)
-            zu_pocket = cp[:, 0:1] * z_pocket + cp[:, 1:2] * ((1 + cp[:, 4:5]) * x0_p - cp[:, 4:5] * hp)
-            mean = scatter_mean(torch.cat((zu_lig[:, :nd], zu_pocket[:, :nd])), torch.cat((lmask, pmask)), dim=0,
-                                dim_size=t.shape[0])
-            for x, m in ((zu_lig, lmask), (zu_pocket, pmask), (x0_l, lmask), (x0_p, pmask), (hl, lmask), (hp, pmask)):
-                x[:, :nd] -= mean[m]
-            hist = (x0_l, x0_p) if commit else (hl, hp)
+            zu_lig, zu_pocket, *hist = self._joint_fast_step(s, t, row, z_lig, z_pocket, *hist, lmask, pmask, sampler, eta, i,
+                                                             commit)
+            hist = tuple(hist)
         # align the COM of the noised known part with the denoised one (en_diffusion.py:751-772)
         shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
             self._fixed_com(zk_lig[:, :nd], zk_pocket[:, :nd], lsel, psel, lmask, pmask)
@@ -964,19 +932,20 @@ class EnVariationalDiffusion(nn.Module):
 
     def _joint_renoise(self, z_lig, z_pocket, hist, gamma_t, gamma_s, lmask, pmask):
         """sample_p_zt_given_zs (the jump back, en_diffusion.py:790-807) with the multistep history ``hist`` (or ()) moved by
-        the same joint COM removal: (lig, pocket) pairs, as _joint_fast_inpaint_step keeps them."""
+        the same joint COM removal: (hist_lig, hist_pocket), as _joint_fast_inpaint_step keeps it."""
         if not hist:
             return (*self.sample_p_zt_given_zs(z_lig, z_pocket, lmask, pmask, gamma_t, gamma_s), ())
+        hl, hp = hist
         nd = self.n_dims
         _, sigma_ts, alpha_ts = self.sigma_and_alpha_t_given_s(gamma_t, gamma_s, z_lig)
         zl, zp = self.sample_normal(alpha_ts[lmask] * z_lig, alpha_ts[pmask] * z_pocket, sigma_ts, lmask, pmask)
         mean = scatter_mean(torch.cat((zl[:, :nd], zp[:, :nd])), torch.cat((lmask, pmask)), dim=0)
-        moved = []
-        for x, m in ((zl, lmask), (zp, pmask)) + tuple(zip(hist, (lmask, pmask) * (len(hist) // 2))):
+
+        def move(x, m):
             x = x.clone()
             x[:, :nd] = x[:, :nd] - mean[m]
-            moved.append(x)
-        return moved[0], moved[1], tuple(moved[2:])
+            return x
+        return (move(zl, lmask), move(zp, pmask), (tuple(move(x, lmask) for x in hl), tuple(move(x, pmask) for x in hp)))
 
     @follows_dynamics_determinism
     @torch.no_grad()
@@ -1052,9 +1021,9 @@ class EnVariationalDiffusion(nn.Module):
 
     @staticmethod
     def _empty_history(x, sampler):
-        """The zero history of one part for the eager multistep steps: one tensor, or the pair (m1, m2) for 'dpmpp_3m'."""
-        h = torch.zeros_like(x)
-        return (h, h) if sampler == 'dpmpp_3m' else h
+        """The zero history of one part for the eager steps, x0_hat tensors newest first: (m1,) for 'dpmpp_2m', (m1, m2) for
+        'dpmpp_3m', () for the samplers without one."""
+        return (torch.zeros_like(x),) * {'dpmpp_2m': 1, 'dpmpp_3m': 2}.get(sampler, 0)
 
     # ---- RePaint-style inpainting with the joint model (en_diffusion.py:653-837) ---------------------------------
     @staticmethod
@@ -1177,9 +1146,10 @@ class EnVariationalDiffusion(nn.Module):
                                 t_back = torch.full((n_samples, 1), fill_value=s + jump_length, device=z_lig.device) / timesteps
                                 g_t = self.inflate_batch_array(self.gamma(t_back), ligand['x'])
                                 g_s = self.inflate_batch_array(self.gamma(s_arr), ligand['x'])
-                                hist = st.get('hist', ()) + st.get('hist2', ())
+                                hists = self._joint_static_history(st)
+                                hist = (tuple(h[0] for h in hists), tuple(h[1] for h in hists)) if hists else ()
                                 zl, zp, moved = self._joint_renoise(st['zl'], st['zp'], hist, g_t, g_s, lmask, pmask)
-                                for x, y in zip(hist, moved):
+                                for x, y in zip(sum(hist, ()), sum(moved, ())):
                                     x.copy_(y)
                                 st['zl'].copy_(zl); st['zp'].copy_(zp); st['step'].add_(jump_length)
                                 if st['seeded']:
@@ -1195,8 +1165,8 @@ class EnVariationalDiffusion(nn.Module):
             if sampler != 'ddpm':
                 t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
             hist = ()
-            if sampler in MULTISTEP:          # one (lig, pocket) pair per history: 2M keeps one, 3M two
-                hist = (torch.zeros_like(z_lig), torch.zeros_like(z_pocket)) * (2 if sampler == 'dpmpp_3m' else 1)
+            if sampler in MULTISTEP:
+                hist = (self._empty_history(z_lig, sampler), self._empty_history(z_pocket, sampler))
             for i, n_denoise in enumerate(schedule):
                 for j in range(n_denoise):
                     jump = j == n_denoise - 1 and i < len(schedule) - 1

@@ -205,7 +205,7 @@ def test_eager_joint_rounds_against_float64():
     fp[::4] = 0
     xl, xp = torch.cat([ligand['x'], ligand['one_hot']], 1), torch.cat([pocket['x'], pocket['one_hot']], 1)
     zl, zp = ddpm.sample_combined_position_feature_noise(lm, pm)
-    hist = (torch.zeros_like(zl), torch.zeros_like(zp)) * 2
+    hist = (ddpm._empty_history(zl, 'dpmpp_3m'), ddpm._empty_history(zp, 'dpmpp_3m'))
     t_table, coef = ddpm._fast_tables(N_STEPS, 'dpmpp_3m', 0.0, 'cpu')
     _, anc = ddpm._joint_tables(N_STEPS, 1, 'cpu')
     noises = []
@@ -225,10 +225,11 @@ def test_eager_joint_rounds_against_float64():
             if not commit:
                 zl1, zp1, h1 = ddpm._joint_renoise(zl1, zp1, h1, ddpm.gamma((sa + 1) / N_STEPS), gs, lm, pm)
             assert len(noises) == 1 + (not commit), 'draws: known part, jump back'
-            args = (zl, zp, *hist, *rec.out, as_kernel(noises[0]), None if commit else as_kernel(noises[1]),
+            (m1l, m2l), (m1p, m2p) = hist
+            args = (zl, zp, m1l, m1p, m2l, m2p, *rec.out, as_kernel(noises[0]), None if commit else as_kernel(noises[1]),
                     coef[s:s + 1].expand(2, -1), anc[s:s + 1, 3:].expand(2, -1), xl, xp, fixed, fp, lm, pm, commit)
             refs = [joint_round3_ref(*args, d) for d in (torch.float32, torch.float64)]
-            got = (zl1, zp1) + tuple(h1)
+            got = (zl1, zp1, h1[0][0], h1[1][0], h1[0][1], h1[1][1])
             for i, name in enumerate(('z_lig', 'z_pocket', 'm1_lig', 'm1_pocket', 'm2_lig', 'm2_pocket')):
                 assert_fp64_bound(got[i], refs[0][i], refs[1][i], f'3M s={s} u={u} {name}')
             zl, zp, hist = zl1, zp1, h1

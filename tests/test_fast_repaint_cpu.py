@@ -143,7 +143,7 @@ def test_eager_conditional_rounds_against_float64(sampler, eta):
     com0 = scatter_mean(pocket['x'], pm, dim=0)
     z = torch.randn(len(lm), 3 + DDPM_CFG.atom_nf)
     z[:, :3], xh_pocket[:, :3] = ddpm.remove_mean_batch(z[:, :3], xh_pocket[:, :3], lm, pm)
-    hist = torch.zeros_like(z)
+    hist = ddpm._empty_history(z, sampler)
     t_table, coef = ddpm._fast_tables(N_STEPS, sampler, eta, 'cpu')
     _, anc = ddpm._schedule_tables(N_STEPS, N_STEPS, 'cpu')
     noises = []
@@ -159,13 +159,16 @@ def test_eager_conditional_rounds_against_float64(sampler, eta):
                                           com0, fixed.view(-1, 1), lm, pm, sampler, eta, last)
             k = int(sampler == 'ddim' and eta > 0)
             assert len(noises) == k + 1 + (not last), 'draws: reverse (DDIM, eta > 0), known part, re-noise'
-            args = (z, xh_pocket, hist, rec.out[0], noises[0] if k else None, noises[k], None if last else noises[k + 1],
+            h = hist[0] if hist else torch.zeros_like(z)
+            args = (z, xh_pocket, h, rec.out[0], noises[0] if k else None, noises[k], None if last else noises[k + 1],
                     coef[s:s + 1].expand(2, -1), anc[s:s + 1, 3:].expand(2, -1), xh_ligand, com0, fixed, lm, pm, sampler, last)
             refs = [cond_round_ref(*args, d) for d in (torch.float32, torch.float64)]
-            for i, name in enumerate(('z', 'pocket', 'hist')[:3 if sampler == 'dpmpp_2m' else 2]):
-                assert_fp64_bound(out[i], refs[0][i], refs[1][i], f'{sampler} eta={eta} s={s} u={u} {name}')
+            got = out[:2] + out[2]
+            assert len(got) == (3 if sampler == 'dpmpp_2m' else 2)
+            for i, name in enumerate(('z', 'pocket', 'hist')[:len(got)]):
+                assert_fp64_bound(got[i], refs[0][i], refs[1][i], f'{sampler} eta={eta} s={s} u={u} {name}')
             if sampler == 'dpmpp_2m' and not last:
-                before, after = _offsets(hist, xh_pocket, lm, pm), _offsets(out[2], out[1], lm, pm)
+                before, after = _offsets(h, xh_pocket, lm, pm), _offsets(out[2][0], out[1], lm, pm)
                 assert float((after - before).abs().max()) <= 1e-5, 'a round that does not commit moved hist against the pocket'
             z, xh_pocket, hist = out
 
@@ -181,7 +184,7 @@ def test_eager_joint_rounds_against_float64(sampler, eta):
     fp = _joint_fixed(pocket)
     xl, xp = torch.cat([ligand['x'], ligand['one_hot']], 1), torch.cat([pocket['x'], pocket['one_hot']], 1)
     zl, zp = ddpm.sample_combined_position_feature_noise(lm, pm)
-    hist = (torch.zeros_like(zl), torch.zeros_like(zp)) if sampler == 'dpmpp_2m' else ()
+    hist = ((torch.zeros_like(zl),), (torch.zeros_like(zp),)) if sampler == 'dpmpp_2m' else ()
     t_table, coef = ddpm._fast_tables(N_STEPS, sampler, eta, 'cpu')
     _, anc = ddpm._joint_tables(N_STEPS, 1, 'cpu')
     noises = []
@@ -202,19 +205,19 @@ def test_eager_joint_rounds_against_float64(sampler, eta):
                 zl1, zp1, h1 = ddpm._joint_renoise(zl1, zp1, h1, ddpm.gamma((sa + 1) / N_STEPS), gs, lm, pm)
             k = int(sampler == 'ddim' and eta > 0)
             assert len(noises) == k + 1 + (not commit), 'draws: known part, reverse (DDIM, eta > 0), jump back'
-            hl, hp = hist if hist else (torch.zeros_like(zl), torch.zeros_like(zp))
+            hl, hp = (hist[0][0], hist[1][0]) if hist else (torch.zeros_like(zl), torch.zeros_like(zp))
             args = (zl, zp, hl, hp, rec.out[0], rec.out[1], as_kernel(noises[1]) if k else None, as_kernel(noises[0]),
                     None if commit else as_kernel(noises[k + 1]), coef[s:s + 1].expand(2, -1), anc[s:s + 1, 3:].expand(2, -1),
                     xl, xp, fixed, fp, lm, pm, sampler, commit)
             refs = [joint_round_ref(*args, d) for d in (torch.float32, torch.float64)]
-            got = (zl1, zp1) + tuple(h1)
+            got = (zl1, zp1) + sum(h1, ())
             for i, name in enumerate(('z_lig', 'z_pocket', 'hist_lig', 'hist_pocket')[:len(got)]):
                 assert_fp64_bound(got[i], refs[0][i], refs[1][i], f'{sampler} eta={eta} s={s} u={u} {name}')
             if sampler == 'dpmpp_2m' and not commit:    # the history is only translated, one shift per graph for all its nodes
-                move = torch.cat((h1[0][:, :3] - hl[:, :3], h1[1][:, :3] - hp[:, :3])).double()
+                move = torch.cat((h1[0][0][:, :3] - hl[:, :3], h1[1][0][:, :3] - hp[:, :3])).double()
                 cm = torch.cat((lm, pm))
                 assert float((move - scatter_mean(move, cm)[cm]).abs().max()) <= 1e-5
-                assert torch.equal(h1[0][:, 3:], hl[:, 3:]) and torch.equal(h1[1][:, 3:], hp[:, 3:])
+                assert torch.equal(h1[0][0][:, 3:], hl[:, 3:]) and torch.equal(h1[1][0][:, 3:], hp[:, 3:])
             zl, zp, hist = zl1, zp1, h1
 
 

@@ -114,7 +114,7 @@ def test_eager_conditional_steps_against_float64(sampler, eta):
     xh_pocket = torch.cat([pocket['x'], pocket['one_hot']], 1)
     z = torch.randn(sum(n_lig), 3 + DDPM_CFG.atom_nf)
     z[:, :3], xh_pocket[:, :3] = ddpm.remove_mean_batch(z[:, :3], xh_pocket[:, :3], lm, pm)
-    hist = torch.zeros_like(z)
+    hist = ddpm._empty_history(z, sampler)
     t_table, coef = ddpm._fast_tables(N_STEPS, sampler, eta, 'cpu')
     noises = []
     lig_noise = ddpm._lig_noise
@@ -127,10 +127,9 @@ def test_eager_conditional_steps_against_float64(sampler, eta):
         assert len(noises) == (1 if eta > 0 else 0)
         if sampler == 'ddim':
             refs = [ddim_ref(z, eps, noises[0] if noises else None, c, xh_pocket, lm, pm, d) for d in (torch.float32, torch.float64)]
-            got = (z1, p1)
         else:
-            refs = [multistep_ref(z, eps, hist, c, xh_pocket, lm, pm, d) for d in (torch.float32, torch.float64)]
-            got = (z1, p1, h1)
+            refs = [multistep_ref(z, eps, *hist, c, xh_pocket, lm, pm, d) for d in (torch.float32, torch.float64)]
+        got = (z1, p1) + h1
         for k, name in enumerate(('z', 'pocket', 'hist')[:len(got)]):
             assert_fp64_bound(got[k], refs[0][k], refs[1][k], f'{sampler} eta={eta} s={s} {name}')
         z, xh_pocket, hist = z1, p1, h1
@@ -144,7 +143,7 @@ def test_eager_joint_steps_against_float64(sampler, eta):
     n_lig, n_poc = [6, 4], [9, 12]
     lm, pm = num_nodes_to_batch_mask(2, torch.tensor(n_lig), 'cpu'), num_nodes_to_batch_mask(2, torch.tensor(n_poc), 'cpu')
     zl, zp = ddpm.sample_combined_position_feature_noise(lm, pm)
-    hl, hp = torch.zeros_like(zl), torch.zeros_like(zp)
+    hl, hp = ddpm._empty_history(zl, sampler), ddpm._empty_history(zp, sampler)
     t_table, coef = ddpm._fast_tables(N_STEPS, sampler, eta, 'cpu')
     noises = []
     draw = ddpm.sample_combined_position_feature_noise
@@ -162,9 +161,11 @@ def test_eager_joint_steps_against_float64(sampler, eta):
                 nz = (torch.cat((el[:, :3], ep[:, :3])), el[:, 3:], ep[:, 3:])
             refs = [joint_ddim_ref(zl, zp, eps_l, eps_p, nz, c, lm, pm, d) for d in (torch.float32, torch.float64)]
         else:
-            refs = [joint_multistep_ref(zl, zp, eps_l, eps_p, hl, hp, c, lm, pm, d) for d in (torch.float32, torch.float64)]
+            refs = [joint_multistep_ref(zl, zp, eps_l, eps_p, *hl, *hp, c, lm, pm, d) for d in (torch.float32, torch.float64)]
+        got = out[:2] + out[2] + out[3]
+        assert len(got) == len(refs[0])
         for k, name in enumerate(('z_lig', 'z_pocket', 'hist_lig', 'hist_pocket')[:len(refs[0])]):
-            assert_fp64_bound(out[k], refs[0][k], refs[1][k], f'{sampler} eta={eta} s={s} {name}')
+            assert_fp64_bound(got[k], refs[0][k], refs[1][k], f'{sampler} eta={eta} s={s} {name}')
         zl, zp, hl, hp = out
 
 
