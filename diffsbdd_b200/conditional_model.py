@@ -187,61 +187,71 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return st
 
     def _captured_step(self, st, kind):
-        """One iteration as a python callable over the static buffers of ``st``.
-        kind: 'reverse' (z_t -> z_s, step -= 1) | 'inpaint_renoise' (reverse step + RePaint blend + re-noise to t) |
-        'inpaint_last' (reverse step + blend, step -= 1) | 'ddim' | 'dpmpp_2m' | 'dpmpp_3m' (_fast_captured_step).  The inpainting kinds
-        of an engine built for a few-step sampler are _fast_inpaint_captured_step."""
-        if kind in ('ddim',) + MULTISTEP:
-            return self._fast_captured_step(st, kind)
-        if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
-            return self._fast_inpaint_captured_step(st, kind)
+        """One iteration as a python callable over the static buffers of ``st``, with the step of the sampler the engine was
+        built for.  kind: 'reverse' ('ddpm') | 'ddim' | 'dpmpp_2m' | 'dpmpp_3m' (z_t -> z_s, step -= 1) | 'inpaint_renoise'
+        (the step + RePaint blend + re-noise to t, u += 1; 2M / 3M: the round does not commit) | 'inpaint_last' (the step +
+        blend, step -= 1, u = 0; 2M / 3M: the last round of the step commits its x0_hat as the history) (DESIGN §13-15).
+        A run: draw ids -> the step's table rows -> native denoiser -> draws -> dsb_ddpm_ligand_update (+
+        dsb_ddpm_inpaint_update), or the 2M / 3M step or RePaint round (_native.multistep_update) -> counters."""
         dyn: EGNNDynamics = self.dynamics
         lib = _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['z'].shape[0], st['pocket'].shape[0]
-
-        def draw(out, purpose):
-            seeded.fill(out, _native.RNG_LIGAND, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
+        sizes = (st['z'].shape[0], st['pocket'].shape[0], n, self.atom_nf, self.residue_nf)
+        ptr = lambda x: None if x is None else x.data_ptr()
+        sampler = st.get('sampler', 'ddpm')
+        repaint, renoise = kind.startswith('inpaint'), kind == 'inpaint_renoise'
+        # table rows -> the buffers the kernels read, {table: [(buffer, first column)]}; one index_select per table
+        coef = 'coef3' if sampler == 'ddpm' else 'coef_fast'
+        if repaint and sampler in MULTISTEP:      # the 2M / 3M row and the RePaint row in one [n, 9 | 10] buffer
+            coef = 'coef9' if sampler == 'dpmpp_2m' else 'coef10'
+            stage = {'ms_table': [(coef, 0)]}
+        else:
+            stage = {'coef_table' if sampler == 'ddpm' else 'fast_table': [(coef, 0)]}
+            if repaint:                           # the RePaint row of dsb_ddpm_inpaint_update
+                stage.setdefault('coef_table', []).append(('coef4', 3))
+        t_table = 't_table' if sampler == 'ddpm' else 'fast_t'     # fast_t: diversify's top moves the few-step grid
+        # the step's draws in eager order: reverse noise ('ddpm', DDIM at eta > 0), known part, re-noise
+        draws = [(p, buf) for p, buf, on in ((seeded.PURPOSE_REVERSE, 'noise', sampler == 'ddpm' or st.get('eta', 0) > 0),
+                                             (seeded.PURPOSE_KNOWN, 'noise1', repaint),
+                                             (seeded.PURPOSE_RENOISE, 'noise2', renoise)) if on]
 
         def run():
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            if st['seeded']:
+            if st['seeded'] and draws:
                 seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
             idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
-            row = st['coef_table'].index_select(0, idx)
-            st['coef3'].copy_(row[:, :3].expand(n, 3))
-            st['coef4'].copy_(row[:, 3:].expand(n, 4))
+            st['t'].copy_(st[t_table].index_select(0, idx).expand(n, 1))
+            for table, bufs in stage.items():
+                row = st[table].index_select(0, idx)
+                for key, c0 in bufs:
+                    st[key].copy_(row[:, c0:c0 + st[key].shape[1]].expand_as(st[key]))
             eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
-            if st['seeded']:
-                draw(st['noise'], seeded.PURPOSE_REVERSE)
-            else:
-                st['noise'].normal_()
-            _native.check(lib.dsb_ddpm_ligand_update(
-                st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef3'].data_ptr(),
-                lm.data_ptr(), pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf,
-                st['z'].data_ptr(), st['pocket'].data_ptr(), stream))
-            if kind != 'reverse':
-                ip = st['inpaint']
-                renoise = kind == 'inpaint_renoise'
+            for p, buf in draws:
                 if st['seeded']:
-                    draw(st['noise1'], seeded.PURPOSE_KNOWN)
-                    if renoise:
-                        draw(st['noise2'], seeded.PURPOSE_RENOISE)
+                    seeded.fill(st[buf], _native.RNG_LIGAND, st['seeds'], st['draw'][p:p + 1], lm, pm)
                 else:
-                    st['noise1'].normal_()
-                    if renoise:
-                        st['noise2'].normal_()
-                _native.check(lib.dsb_ddpm_inpaint_update(
-                    st['z'].data_ptr(), st['pocket'].data_ptr(), ip['known'].data_ptr(), ip['com0'].data_ptr(),
-                    ip['fixed'].data_ptr(), st['noise1'].data_ptr(), st['noise2'].data_ptr() if renoise else None,
-                    st['coef4'].data_ptr(), lm.data_ptr(), pm.data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            if kind != 'inpaint_renoise':
-                st['step'].sub_(1)
-            if st['seeded'] and kind != 'reverse':
-                if kind == 'inpaint_renoise':
+                    st[buf].normal_()
+            ip = st['inpaint']
+            n2 = st['noise2'] if renoise else None
+            if sampler in MULTISTEP:
+                rp = ((ip['known'], None, ip['com0'], ip['fixed'], None, st['noise1'], None, None, n2, None, None) if repaint
+                      else ())
+                _native.multistep_update(lib, (st['z'], st['pocket']), self._static_history(st), (eps, None), st[coef],
+                                         (lm, pm), sizes, 0, stream, rp, int(not renoise))
+            else:
+                _native.check(lib.dsb_ddpm_ligand_update(
+                    ptr(st['z']), ptr(eps), ptr(st['noise']), ptr(st[coef]), ptr(lm), ptr(pm), ptr(st['pocket']), *sizes,
+                    ptr(st['z']), ptr(st['pocket']), stream))
+                if repaint:
+                    _native.check(lib.dsb_ddpm_inpaint_update(
+                        ptr(st['z']), ptr(st['pocket']), ptr(ip['known']), ptr(ip['com0']), ptr(ip['fixed']), ptr(st['noise1']),
+                        ptr(n2), ptr(st['coef4']), ptr(lm), ptr(pm), *sizes, stream))
+            if renoise:
+                if st['seeded']:
                     st['u'].add_(1)
-                else:
+            else:
+                st['step'].sub_(1)
+                if st['seeded'] and kind == 'inpaint_last':
                     st['u'].zero_()
         return run
 
@@ -312,39 +322,6 @@ class ConditionalDDPM(EnVariationalDiffusion):
         dyn.check_status()
         return st['z'].clone(), st['pocket'].clone()
 
-    def _fast_captured_step(self, st, kind):
-        """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step over the static buffers of ``st`` (step -= 1): table row of the step
-        counter -> native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients (noise drawn only at eta > 0), or the
-        2M / 3M step (_native.multistep_update)."""
-        dyn: EGNNDynamics = self.dynamics
-        lib = _native.load()
-        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['z'].shape[0], st['pocket'].shape[0]
-        k = st['fast_table'].shape[1]
-
-        def run():
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['fast_t'].index_select(0, idx).expand(n, 1))
-            st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, k))
-            eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
-            if kind == 'ddim':
-                if st['eta'] > 0 and st['seeded']:
-                    seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
-                    seeded.fill(st['noise'], _native.RNG_LIGAND, st['seeds'],
-                                st['draw'][seeded.PURPOSE_REVERSE:seeded.PURPOSE_REVERSE + 1], lm, pm)
-                elif st['eta'] > 0:
-                    st['noise'].normal_()
-                _native.check(lib.dsb_ddpm_ligand_update(
-                    st['z'].data_ptr(), eps.data_ptr(), st['noise'].data_ptr(), st['coef_fast'].data_ptr(), lm.data_ptr(),
-                    pm.data_ptr(), st['pocket'].data_ptr(), NL, NP, n, self.atom_nf, self.residue_nf, st['z'].data_ptr(),
-                    st['pocket'].data_ptr(), stream))
-            else:
-                _native.multistep_update(lib, (st['z'], st['pocket']), self._static_history(st), (eps, None), st['coef_fast'],
-                                         (lm, pm), (NL, NP, n, self.atom_nf, self.residue_nf), 0, stream)
-            st['step'].sub_(1)
-        return run
-
     def _graphed_fast_loop(self, z_lig, xh_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta, return_frames,
                            out_lig, out_pocket, top=None):
         """The whole 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' reverse loop as ``timesteps`` replays of one captured step; frames are
@@ -369,10 +346,14 @@ class ConditionalDDPM(EnVariationalDiffusion):
         return st['z'].clone(), st['pocket'].clone()
 
     def _fast_step(self, s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket_mask, sampler, eta, u=0, commit=True):
-        """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s (DESIGN §13, §15); ``row`` [1, k]: the step's row of
-        _fast_tables; ``hist``: the history (_empty_history).  Returns (z_lig, xh_pocket, hist): with ``commit`` the history
-        multistep_update writes, else the one given; either way moved by the step's ligand-COM removal, so that it stays in
-        the pocket's frame.  ``u``: the resampling round of the seeded DDIM draw (RePaint)."""
+        """Eager step z_t -> z_s of any sampler (DESIGN §13, §15): 'ddpm' is sample_p_zs_given_zt at s = ``row`` (the s/T
+        array) and t; for 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' ``row`` [1, k] is the step's row of _fast_tables.  ``hist``: the
+        history (_empty_history).  Returns (z_lig, xh_pocket, hist): with ``commit`` the history multistep_update writes, else
+        the one given; either way moved by the step's ligand-COM removal, so that it stays in the pocket's frame.  ``u``: the
+        resampling round of the seeded reverse draw (RePaint)."""
+        if sampler == 'ddpm':
+            self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
+            return (*self.sample_p_zs_given_zt(row, t, z_lig, xh_pocket, lig_mask, pocket_mask), hist)
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
         cl = c[lig_mask]
@@ -400,90 +381,20 @@ class ConditionalDDPM(EnVariationalDiffusion):
             h[:, :nd] = moved[NP + k * NL:NP + (k + 1) * NL]
         return z_lig, xh_pocket, hist
 
-    def _fast_inpaint_captured_step(self, st, kind):
-        """One RePaint round of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15); kind as _captured_step
-        ('inpaint_renoise': re-noised, the round does not commit; 'inpaint_last': the last round of the step, which commits
-        its x0_hat as the 2M / 3M history).  DDIM: native denoiser -> dsb_ddpm_ligand_update with the DDIM coefficients ->
-        dsb_ddpm_inpaint_update.  2M / 3M: native denoiser -> the fused RePaint round (_native.multistep_update)."""
-        dyn: EGNNDynamics = self.dynamics
-        lib = _native.load()
-        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['z'].shape[0], st['pocket'].shape[0]
-        renoise = kind == 'inpaint_renoise'
-        ddim = st['sampler'] == 'ddim'
-        ms_key = 'coef9' if st['sampler'] == 'dpmpp_2m' else 'coef10'      # the 2M / 3M row + the RePaint row
-
-        def draw(out, purpose):
-            if st['seeded']:
-                seeded.fill(out, _native.RNG_LIGAND, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
-            else:
-                out.normal_()
-
-        def run():
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            ptr = lambda x: x.data_ptr()
-            if st['seeded']:
-                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
-            idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['fast_t'].index_select(0, idx).expand(n, 1))
-            if ddim:
-                st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
-                st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
-            else:
-                st[ms_key].copy_(st['ms_table'].index_select(0, idx).expand(n, st['ms_table'].shape[1]))
-            eps, _ = dyn(st['z'], st['pocket'], st['t'], lm, pm)
-            if ddim and st['eta'] > 0:
-                draw(st['noise'], seeded.PURPOSE_REVERSE)
-            draw(st['noise1'], seeded.PURPOSE_KNOWN)
-            if renoise:
-                draw(st['noise2'], seeded.PURPOSE_RENOISE)
-            ip = st['inpaint']
-            if ddim:
-                n2 = ptr(st['noise2']) if renoise else None
-                _native.check(lib.dsb_ddpm_ligand_update(
-                    ptr(st['z']), ptr(eps), ptr(st['noise']), ptr(st['coef_fast']), ptr(lm), ptr(pm), ptr(st['pocket']), NL, NP,
-                    n, self.atom_nf, self.residue_nf, ptr(st['z']), ptr(st['pocket']), stream))
-                _native.check(lib.dsb_ddpm_inpaint_update(
-                    ptr(st['z']), ptr(st['pocket']), ptr(ip['known']), ptr(ip['com0']), ptr(ip['fixed']), ptr(st['noise1']), n2,
-                    ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            else:
-                _native.multistep_update(
-                    lib, (st['z'], st['pocket']), self._static_history(st), (eps, None), st[ms_key], (lm, pm),
-                    (NL, NP, n, self.atom_nf, self.residue_nf), 0, stream,
-                    (ip['known'], None, ip['com0'], ip['fixed'], None, st['noise1'], None, None,
-                     st['noise2'] if renoise else None, None, None), int(not renoise))
-            if renoise:
-                if st['seeded']:
-                    st['u'].add_(1)
-            else:
-                st['step'].sub_(1)
-                if st['seeded']:
-                    st['u'].zero_()
-        return run
-
     def _fast_inpaint_step(self, s, u, t, row, gamma_s, gamma_t, z_lig, xh_pocket, hist, ligand_x, xh_ligand, com_pocket_0,
                            lig_fixed, lmask, pmask, sampler, eta, last):
-        """Eager RePaint round (s, u) of _inpaint (DESIGN §14): the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row``
-        and t; 'ddim' / 'dpmpp_2m' / 'dpmpp_3m': the few-step step with ``row`` [1, k], the step's row of _fast_tables), then
+        """Eager RePaint round (s, u) of _inpaint (DESIGN §14): the reverse step (_fast_step with ``t`` and ``row``), then
         the known part, the COM alignment, the blend and, unless ``last``, the re-noising.  ``hist`` (_empty_history) is the
         history committed by the last round of step s + 1, kept in the pocket's frame: every translation of the pocket
         coordinates moves it too, and the last round of step s commits its own (multistep_update); 'ddpm' and DDIM leave it
         as it is.  Returns (z_lig, xh_pocket, hist)."""
         nd, NL, NP = self.n_dims, z_lig.shape[0], xh_pocket.shape[0]
         fixed_rows = lig_fixed.bool().view(-1)
-        hists = ()          # the multistep history, moved by the step
-        if sampler == 'ddpm':
-            self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
-            z_unknown, xh_pocket = self.sample_p_zs_given_zt(row, t, z_lig, xh_pocket, lmask, pmask)
-        elif sampler == 'ddim':
-            z_unknown, xh_pocket, _ = self._fast_step(s, t, row, z_lig, xh_pocket, (), lmask, pmask, sampler, eta, u)
-        else:
-            z_unknown, xh_pocket, hists = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u,
-                                                          last)
+        z_unknown, xh_pocket, hist = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lmask, pmask, sampler, eta, u, last)
         # frame: the rows that every pocket translation moves (the pocket's x columns and the history), under the pocket's
         # graph index
-        frame = torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hists))
-        fmask = torch.cat((pmask,) + (lmask,) * len(hists))
+        frame = torch.cat((xh_pocket[:, :nd],) + tuple(h[:, :nd] for h in hist))
+        fmask = torch.cat((pmask,) + (lmask,) * len(hist))
 
         # noise the known part to level s, following the pocket's current COM (conditional_model.py:636-643)
         com_pocket = scatter_mean(frame[:NP], pmask, dim=0)
@@ -501,8 +412,7 @@ class ConditionalDDPM(EnVariationalDiffusion):
             self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_RENOISE)
             z_lig, frame = self.sample_p_zt_given_zs(z_lig, frame, lmask, fmask, gamma_t, gamma_s)
         xh_pocket = torch.cat((frame[:NP], xh_pocket[:, nd:]), dim=1)
-        if hists:
-            hist = tuple(torch.cat((frame[NP + k * NL:NP + (k + 1) * NL], h[:, nd:]), dim=1) for k, h in enumerate(hists))
+        hist = tuple(torch.cat((frame[NP + k * NL:NP + (k + 1) * NL], h[:, nd:]), dim=1) for k, h in enumerate(hist))
         return z_lig, xh_pocket, hist
 
     def _graphed_inpaint_loop(self, z_lig, xh_pocket, xh_known, com_pocket_0, lig_fixed, lmask, pmask, n_samples,
@@ -574,21 +484,11 @@ class ConditionalDDPM(EnVariationalDiffusion):
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + xh_pocket.size(), device=device)
 
-        if sampler != 'ddpm' and self._use_graph(device):
+        use_graph = self._use_graph(device)
+        if use_graph and sampler != 'ddpm':
             z_lig, xh_pocket = self._graphed_fast_loop(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples, timesteps, sampler,
                                                        eta, return_frames, out_lig, out_pocket)
-            self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
-        elif sampler != 'ddpm':
-            t_table, coef = self._fast_tables(timesteps, sampler, eta, device)
-            hist = self._empty_history(z_lig, sampler)
-            for s in reversed(range(0, timesteps)):
-                z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
-                                                         hist, lig_mask, pocket['mask'], sampler, eta)
-                if (s * return_frames) % timesteps == 0:
-                    idx = (s * return_frames) // timesteps
-                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
-            self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
-        elif self._use_graph(device):
+        elif use_graph:
             stride = timesteps // return_frames       # frames are saved at s = idx * stride
             s_hi = timesteps - 1
             while s_hi >= 0:
@@ -597,17 +497,17 @@ class ConditionalDDPM(EnVariationalDiffusion):
                     z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples, s_hi, s_hi - s_lo + 1, timesteps)
                 out_lig[s_lo // stride], out_pocket[s_lo // stride] = self.unnormalize_z(z_lig, xh_pocket)
                 s_hi = s_lo - 1
-            self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
         else:
+            fast = None if sampler == 'ddpm' else self._fast_tables(timesteps, sampler, eta, device)
+            hist = self._empty_history(z_lig, sampler)
             for s in reversed(range(0, timesteps)):
-                s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
-                t_array = (s_array + 1) / timesteps
-                s_array = s_array / timesteps
-                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
-                z_lig, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig, xh_pocket, lig_mask, pocket['mask'])
+                t, row = self._eager_row(s, timesteps, n_samples, device, fast)
+                z_lig, xh_pocket, hist = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket['mask'], sampler,
+                                                         eta)
                 if (s * return_frames) % timesteps == 0:
                     idx = (s * return_frames) // timesteps
                     out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, xh_pocket)
+        self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
 
         self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples)
@@ -835,27 +735,22 @@ class ConditionalDDPM(EnVariationalDiffusion):
         lig_mask = ligand['mask']
         self.assert_mean_zero_with_mask(z_lig[:, :self.n_dims], lig_mask)
         top = (noising_steps, timesteps)
-        if sampler != 'ddpm' and self._use_graph(z_lig.device) and noising_steps > 0:
-            frame = torch.empty((1,) + z_lig.shape, device=z_lig.device), torch.empty((1,) + xh_pocket.shape, device=z_lig.device)
+        device = z_lig.device
+        use_graph = self._use_graph(device) and noising_steps > 0
+        if use_graph and sampler != 'ddpm':
+            frame = torch.empty((1,) + z_lig.shape, device=device), torch.empty((1,) + xh_pocket.shape, device=device)
             z_lig, xh_pocket = self._graphed_fast_loop(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples, denoising_steps,
                                                        sampler, eta, 1, *frame, top=top)
-        elif sampler != 'ddpm' and noising_steps > 0:
-            t_table, coef = self._fast_tables(denoising_steps, sampler, eta, z_lig.device, top)
-            hist = self._empty_history(z_lig, sampler)
-            for s in reversed(range(0, denoising_steps)):
-                z_lig, xh_pocket, hist = self._fast_step(s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, xh_pocket,
-                                                         hist, lig_mask, pocket['mask'], sampler, eta)
-        elif self._use_graph(z_lig.device) and noising_steps > 0:
+        elif use_graph:
             z_lig, xh_pocket = self._graphed_reverse_steps(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples,
                                                            noising_steps - 1, noising_steps, timesteps)
-        else:
-            for s in reversed(range(0, noising_steps)):
-                s_array = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
-                t_array = (s_array + 1) / timesteps
-                s_array = s_array / timesteps
-                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
-                z_lig, xh_pocket = self.sample_p_zs_given_zt(s_array, t_array, z_lig.detach(), xh_pocket.detach(),
-                                                             lig_mask, pocket['mask'])
+        elif noising_steps > 0:           # 'ddpm' takes the T grid: denoising_steps = noising_steps
+            fast = None if sampler == 'ddpm' else self._fast_tables(denoising_steps, sampler, eta, device, top)
+            hist = self._empty_history(z_lig, sampler)
+            for s in reversed(range(0, denoising_steps)):
+                t, row = self._eager_row(s, timesteps, n_samples, device, fast)
+                z_lig, xh_pocket, hist = self._fast_step(s, t, row, z_lig, xh_pocket, hist, lig_mask, pocket['mask'], sampler,
+                                                         eta)
         self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, xh_pocket, lig_mask, pocket['mask'], n_samples)
         self.assert_mean_zero_with_mask(x_lig, lig_mask)

@@ -576,6 +576,17 @@ class EnVariationalDiffusion(nn.Module):
         coef = fast_coefficients(self.gamma(s_arr), self.gamma(t_arr), sampler, eta)
         return t_arr.float().contiguous(), coef.float().contiguous()
 
+    @staticmethod
+    def _eager_row(s, timesteps, n_samples, device, fast):
+        """(t, row) of eager step s as _fast_step / _joint_fast_step take them.  'ddpm' (``fast`` None): the reference's
+        t = (s + 1) / timesteps and s / timesteps, [n_samples, 1] each; else t and the step's row [1, k] of ``fast``, the
+        (t, coefficients) pair of _fast_tables."""
+        if fast is None:
+            s_array = torch.full((n_samples, 1), fill_value=s, device=device)
+            return (s_array + 1) / timesteps, s_array / timesteps
+        t_table, coef = fast
+        return t_table[s].expand(n_samples, 1), coef[s:s + 1]
+
     def _joint_engine(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, jump_length, sampler='ddpm', eta=0.0):
         dyn = self.dynamics
         device = z_lig.device
@@ -622,57 +633,68 @@ class EnVariationalDiffusion(nn.Module):
         return st
 
     def _joint_step(self, st, kind):
-        """kind: 'reverse' (sample: one joint reverse step, step -= 1) | 'inpaint' (noised known part + reverse step + blend,
-        step -= 1) | 'inpaint_jump' (the same + jump back by jump_length: step += jump_length - 1) | 'ddim' | 'dpmpp_2m' |
-        'dpmpp_3m' (_joint_fast_captured_step).  The inpainting kinds of an engine built for a few-step sampler, and its 'inpaint_hold',
-        are _joint_fast_inpaint_captured_step."""
+        """One iteration of the joint model as a python callable over the static buffers of ``st``, with the step of the
+        sampler the engine was built for.  kind: 'reverse' ('ddpm') | 'ddim' | 'dpmpp_2m' | 'dpmpp_3m' (one joint step,
+        step -= 1) | 'inpaint' (noised known part + the step + blend, step -= 1; 2M / 3M: commits its x0_hat as the history) |
+        'inpaint_jump' (the same + jump back by jump_length, no commit: step += jump_length - 1, u += 1) | 'inpaint_hold'
+        (as 'inpaint' without the commit: a frame is taken before an eager jump back) (DESIGN §13-15).  A run: draw ids ->
+        the step's table rows -> native denoiser -> draws -> dsb_ddpm_joint_update (+ dsb_ddpm_joint_inpaint_update), or the
+        2M / 3M step or RePaint round (_native.multistep_update) -> counters."""
         import ctypes as C
         from . import _native, seeded
-        if kind in ('ddim',) + MULTISTEP:
-            return self._joint_fast_captured_step(st, kind)
-        if kind != 'reverse' and st.get('sampler', 'ddpm') != 'ddpm':
-            return self._joint_fast_inpaint_captured_step(st, kind)
         dyn, lib = self.dynamics, _native.load()
         lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['zl'].shape[0], st['zp'].shape[0]
-        ptr = lambda x: x.data_ptr()
+        sizes = (st['zl'].shape[0], st['zp'].shape[0], n, self.atom_nf, self.residue_nf)
+        ptr = lambda x: None if x is None else x.data_ptr()
         roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
-
-        def draw(bufs, purpose):
-            if st['seeded']:
-                for x, role in zip(bufs, roles):
-                    seeded.fill(x, role, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
-            else:
-                for x in bufs:
-                    x.normal_()
+        sampler = st.get('sampler', 'ddpm')
+        repaint, jump = kind.startswith('inpaint'), kind == 'inpaint_jump'
+        # table rows -> the buffers the kernels read, {table: [(buffer, first column)]}; one index_select per table
+        coef = 'coef3' if sampler == 'ddpm' else 'coef_fast'
+        if repaint and sampler in MULTISTEP:      # the 2M / 3M row and the RePaint row in one [n, 9 | 10] buffer
+            coef = 'coef9' if sampler == 'dpmpp_2m' else 'coef10'
+            stage = {'ms_table': [(coef, 0)]}
+        else:
+            stage = {'coef_table' if sampler == 'ddpm' else 'fast_table': [(coef, 0)]}
+            if repaint:                           # the RePaint row of dsb_ddpm_joint_inpaint_update
+                stage.setdefault('coef_table', []).append(('coef4', 3))
+        # the step's draws in eager order (en_diffusion.py:741): known part, reverse noise ('ddpm', DDIM at eta > 0), jump
+        draws = [(p, buf) for p, buf, on in ((seeded.PURPOSE_KNOWN, 'n_known', repaint),
+                                             (seeded.PURPOSE_REVERSE, 'n_rev', sampler == 'ddpm' or st.get('eta', 0) > 0),
+                                             (seeded.PURPOSE_RENOISE, 'n_jump', jump)) if on]
 
         def run():
             stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            if st['seeded']:
+            if st['seeded'] and draws:
                 seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
-            if kind != 'reverse':                       # eager order: noised_representation draws first (en_diffusion.py:741)
-                draw(st['n_known'], seeded.PURPOSE_KNOWN)
-            row = st['coef_table'].index_select(0, st['step'].clamp(min=0))
-            st['t'].copy_(st['t_table'].index_select(0, st['step'].clamp(min=0)).expand(n, 1))
-            st['coef3'].copy_(row[:, :3].expand(n, 3))
-            st['coef4'].copy_(row[:, 3:].expand(n, 4))
+            idx = st['step'].clamp(min=0)
+            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
+            for table, bufs in stage.items():
+                row = st[table].index_select(0, idx)
+                for key, c0 in bufs:
+                    st[key].copy_(row[:, c0:c0 + st[key].shape[1]].expand_as(st[key]))
             eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
-            draw(st['n_rev'], seeded.PURPOSE_REVERSE)
-            nx, nhl, nhp = st['n_rev']
-            _native.check(lib.dsb_ddpm_joint_update(
-                ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef3']),
-                ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            if kind != 'reverse':
-                kn = st['known']
-                jump = kind == 'inpaint_jump'
-                if jump:
-                    draw(st['n_jump'], seeded.PURPOSE_RENOISE)
-                j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
-                _native.check(lib.dsb_ddpm_joint_inpaint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
-                    *[ptr(x) for x in st['n_known']], *j, ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n,
-                    self.atom_nf, self.residue_nf, stream))
-            if kind == 'inpaint_jump':
+            for p, buf in draws:
+                for x, role in zip(st[buf], roles):
+                    if st['seeded']:
+                        seeded.fill(x, role, st['seeds'], st['draw'][p:p + 1], lm, pm)
+                    else:
+                        x.normal_()
+            kn = st['known']
+            n_jump = st['n_jump'] if jump else (None,) * 3
+            if sampler in MULTISTEP:
+                rp = (kn['xl'], kn['xp'], None, kn['fl'], kn['fp'], *st['n_known'], *n_jump) if repaint else ()
+                _native.multistep_update(lib, (st['zl'], st['zp']), self._joint_static_history(st), (eps_l, eps_p), st[coef],
+                                         (lm, pm), sizes, 1, stream, rp, int(kind == 'inpaint'))
+            else:
+                _native.check(lib.dsb_ddpm_joint_update(
+                    ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), *map(ptr, st['n_rev']), ptr(st[coef]), ptr(lm),
+                    ptr(pm), *sizes, stream))
+                if repaint:
+                    _native.check(lib.dsb_ddpm_joint_inpaint_update(
+                        ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
+                        *map(ptr, st['n_known']), *map(ptr, n_jump), ptr(st['coef4']), ptr(lm), ptr(pm), *sizes, stream))
+            if jump:
                 st['step'].add_(st['jump'] - 1)
                 if st['seeded']:
                     st['u'].add_(1)
@@ -741,45 +763,6 @@ class EnVariationalDiffusion(nn.Module):
         dyn.check_status()
         return st['zl'].clone(), st['zp'].clone()
 
-    def _joint_fast_captured_step(self, st, kind):
-        """One 'ddim', 'dpmpp_2m' or 'dpmpp_3m' step of the joint model over the static buffers of ``st`` (step -= 1): table
-        row of the step counter -> native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients (noise drawn only at
-        eta > 0), or the 2M / 3M step (_native.multistep_update)."""
-        import ctypes as C
-        from . import _native, seeded
-        dyn, lib = self.dynamics, _native.load()
-        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['zl'].shape[0], st['zp'].shape[0]
-        ptr = lambda x: x.data_ptr()
-        roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
-        k = st['fast_table'].shape[1]
-        rev = slice(seeded.PURPOSE_REVERSE, seeded.PURPOSE_REVERSE + 1)
-
-        def run():
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
-            st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, k))
-            eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
-            if kind == 'ddim':
-                if st['eta'] > 0:
-                    if st['seeded']:
-                        seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
-                        for x, role in zip(st['n_rev'], roles):
-                            seeded.fill(x, role, st['seeds'], st['draw'][rev], lm, pm)
-                    else:
-                        for x in st['n_rev']:
-                            x.normal_()
-                nx, nhl, nhp = st['n_rev']
-                _native.check(lib.dsb_ddpm_joint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
-                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-            else:
-                _native.multistep_update(lib, (st['zl'], st['zp']), self._joint_static_history(st), (eps_l, eps_p),
-                                         st['coef_fast'], (lm, pm), (NL, NP, n, self.atom_nf, self.residue_nf), 1, stream)
-            st['step'].sub_(1)
-        return run
-
     def _graphed_joint_fast_loop(self, z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler, eta,
                                  return_frames, out_lig, out_pocket):
         """The whole 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' reverse loop as ``timesteps`` replays of one captured step; frames are
@@ -802,12 +785,15 @@ class EnVariationalDiffusion(nn.Module):
         return st['zl'].clone(), st['zp'].clone()
 
     def _joint_fast_step(self, s, t, row, zl, zp, hl, hp, lig_mask, pocket_mask, sampler, eta, u=0, commit=True):
-        """Eager 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' step z_t -> z_s of the joint model (DESIGN §13, §15); ``row`` [1, k]: the
-        step's row of _fast_tables.  ``hl``, ``hp``: the history of each part (_empty_history).  Returns (z_lig, z_pocket,
-        hist_lig, hist_pocket): with ``commit`` the history multistep_update writes, else the one given; either way moved
-        by the step's joint COM removal, so that it stays in the frame of z.  ``u``: the RePaint block of the seeded DDIM
-        draw."""
+        """Eager step z_t -> z_s of the joint model for any sampler (DESIGN §13, §15): 'ddpm' is sample_p_zs_given_zt at
+        s = ``row`` (the s/T array) and t; for 'ddim' / 'dpmpp_2m' / 'dpmpp_3m' ``row`` [1, k] is the step's row of
+        _fast_tables.  ``hl``, ``hp``: the history of each part (_empty_history).  Returns (z_lig, z_pocket, hist_lig,
+        hist_pocket): with ``commit`` the history multistep_update writes, else the one given; either way moved by the step's
+        joint COM removal, so that it stays in the frame of z.  ``u``: the RePaint block of the seeded reverse draw."""
         from . import seeded
+        if sampler == 'ddpm':
+            self._draw_at(seeded.STAGE_LOOP, s, u, seeded.PURPOSE_REVERSE)
+            return (*self.sample_p_zs_given_zt(row, t, zl, zp, lig_mask, pocket_mask), hl, hp)
         nd = self.n_dims
         c = row.expand(t.shape[0], -1)
         cl, cp = c[lig_mask], c[pocket_mask]
@@ -832,79 +818,12 @@ class EnVariationalDiffusion(nn.Module):
             x[:, :nd] -= mean[m]
         return zl, zp, hl, hp
 
-    def _joint_fast_inpaint_captured_step(self, st, kind):
-        """One RePaint iteration of an engine built for 'ddim', 'dpmpp_2m' or 'dpmpp_3m' (DESIGN §14, §15).  kind: 'inpaint'
-        (blend; the iteration commits its x0_hat as the 2M / 3M history; step -= 1) | 'inpaint_jump' (blend + jump back, no commit; step +=
-        jump_length - 1) | 'inpaint_hold' (blend, no commit, step -= 1: a frame is taken before an eager jump back).  DDIM:
-        native denoiser -> dsb_ddpm_joint_update with the DDIM coefficients -> dsb_ddpm_joint_inpaint_update.  2M / 3M:
-        native denoiser -> the fused RePaint round (_native.multistep_update)."""
-        import ctypes as C
-        from . import _native, seeded
-        dyn, lib = self.dynamics, _native.load()
-        lm, pm, n = st['lig_mask'], st['pocket_mask'], st['n_samples']
-        NL, NP = st['zl'].shape[0], st['zp'].shape[0]
-        ptr = lambda x: x.data_ptr()
-        roles = (_native.RNG_JOINT_X, _native.RNG_LIGAND, _native.RNG_POCKET)
-        ddim, jump = st['sampler'] == 'ddim', kind == 'inpaint_jump'
-        ms_key = 'coef9' if st['sampler'] == 'dpmpp_2m' else 'coef10'      # the 2M / 3M row + the RePaint row
-
-        def draw(bufs, purpose):
-            if st['seeded']:
-                for x, role in zip(bufs, roles):
-                    seeded.fill(x, role, st['seeds'], st['draw'][purpose:purpose + 1], lm, pm)
-            else:
-                for x in bufs:
-                    x.normal_()
-
-        def run():
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-            if st['seeded']:
-                seeded.graph_draw_ids(st['step'], st['u'], st['draw'])
-            draw(st['n_known'], seeded.PURPOSE_KNOWN)              # eager order: known part, reverse step, jump back
-            idx = st['step'].clamp(min=0)
-            st['t'].copy_(st['t_table'].index_select(0, idx).expand(n, 1))
-            if ddim:
-                st['coef_fast'].copy_(st['fast_table'].index_select(0, idx).expand(n, 3))
-                st['coef4'].copy_(st['coef_table'].index_select(0, idx)[:, 3:].expand(n, 4))
-            else:
-                st[ms_key].copy_(st['ms_table'].index_select(0, idx).expand(n, st['ms_table'].shape[1]))
-            eps_l, eps_p = dyn(st['zl'], st['zp'], st['t'], lm, pm)
-            if ddim and st['eta'] > 0:
-                draw(st['n_rev'], seeded.PURPOSE_REVERSE)
-            if jump:
-                draw(st['n_jump'], seeded.PURPOSE_RENOISE)
-            kn = st['known']
-            if ddim:
-                j = [ptr(x) for x in st['n_jump']] if jump else [None, None, None]
-                nx, nhl, nhp = st['n_rev']
-                _native.check(lib.dsb_ddpm_joint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(eps_l), ptr(eps_p), ptr(nx), ptr(nhl), ptr(nhp), ptr(st['coef_fast']),
-                    ptr(lm), ptr(pm), NL, NP, n, self.atom_nf, self.residue_nf, stream))
-                _native.check(lib.dsb_ddpm_joint_inpaint_update(
-                    ptr(st['zl']), ptr(st['zp']), ptr(kn['xl']), ptr(kn['xp']), ptr(kn['fl']), ptr(kn['fp']),
-                    *[ptr(x) for x in st['n_known']], *j, ptr(st['coef4']), ptr(lm), ptr(pm), NL, NP, n,
-                    self.atom_nf, self.residue_nf, stream))
-            else:
-                _native.multistep_update(
-                    lib, (st['zl'], st['zp']), self._joint_static_history(st), (eps_l, eps_p), st[ms_key], (lm, pm),
-                    (NL, NP, n, self.atom_nf, self.residue_nf), 1, stream,
-                    (kn['xl'], kn['xp'], None, kn['fl'], kn['fp'], *st['n_known'], *(st['n_jump'] if jump else (None,) * 3)),
-                    int(kind == 'inpaint'))
-            if jump:
-                st['step'].add_(st['jump'] - 1)
-                if st['seeded']:
-                    st['u'].add_(1)
-            else:
-                st['step'].sub_(1)
-        return run
-
     def _joint_fast_inpaint_step(self, s, i, t, row, gamma_s, z_lig, z_pocket, hist, xh0_lig, xh0_pocket, lig_fixed,
                                  pocket_fixed, lsel, psel, lmask, pmask, sampler, eta, commit):
         """Eager RePaint iteration (s, block i) of the joint inpaint (DESIGN §14), without the jump back (_joint_renoise): the
-        known part, the reverse step ('ddpm': sample_p_zs_given_zt at s = ``row`` and t; 'ddim' / 'dpmpp_2m': the few-step
-        step with ``row`` [1, k], the step's row of _fast_tables), the COM alignment and the blend.  ``hist``: () for
-        'ddpm' and DDIM; for the multistep samplers (hist_lig, hist_pocket) as _joint_fast_step takes them, committed by the
-        last iteration of step s + 1, in the frame of z.  The multistep COM removal moves it with z; the blend keeps the
+        known part, the reverse step (_joint_fast_step with ``t`` and ``row``), the COM alignment and the blend.  ``hist``:
+        () for 'ddpm' and DDIM; for the multistep samplers (hist_lig, hist_pocket) as _joint_fast_step takes them, committed
+        by the last iteration of step s + 1, in the frame of z.  The multistep COM removal moves it with z; the blend keeps the
         frame of the unknown part, so nothing else moves it; ``commit``: this iteration writes the history
         (multistep_update).  Returns (z_lig, z_pocket, hist)."""
         from . import seeded
@@ -912,15 +831,9 @@ class EnVariationalDiffusion(nn.Module):
         # known nodes: forward-noised data; unknown nodes: one reverse step (en_diffusion.py:741-749)
         self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_KNOWN)
         zk_lig, zk_pocket, _, _ = self.noised_representation(xh0_lig, xh0_pocket, lmask, pmask, gamma_s)
-        if sampler == 'ddpm':
-            self._draw_at(seeded.STAGE_LOOP, s, i, seeded.PURPOSE_REVERSE)
-            zu_lig, zu_pocket = self.sample_p_zs_given_zt(row, t, z_lig, z_pocket, lmask, pmask)
-        elif sampler == 'ddim':
-            zu_lig, zu_pocket, _, _ = self._joint_fast_step(s, t, row, z_lig, z_pocket, (), (), lmask, pmask, sampler, eta, i)
-        else:
-            zu_lig, zu_pocket, *hist = self._joint_fast_step(s, t, row, z_lig, z_pocket, *hist, lmask, pmask, sampler, eta, i,
-                                                             commit)
-            hist = tuple(hist)
+        zu_lig, zu_pocket, hl, hp = self._joint_fast_step(s, t, row, z_lig, z_pocket, *(hist or ((), ())), lmask, pmask, sampler,
+                                                          eta, i, commit)
+        hist = (hl, hp) if hl else ()
         # align the COM of the noised known part with the denoised one (en_diffusion.py:751-772)
         shift = self._fixed_com(zu_lig[:, :nd], zu_pocket[:, :nd], lsel, psel, lmask, pmask) - \
             self._fixed_com(zk_lig[:, :nd], zk_pocket[:, :nd], lsel, psel, lmask, pmask)
@@ -975,22 +888,11 @@ class EnVariationalDiffusion(nn.Module):
         self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         out_lig = torch.zeros((return_frames,) + z_lig.size(), device=z_lig.device)
         out_pocket = torch.zeros((return_frames,) + z_pocket.size(), device=z_pocket.device)
-        if sampler != 'ddpm' and self._joint_use_graph(z_lig.device):
+        use_graph = self._joint_use_graph(z_lig.device)
+        if use_graph and sampler != 'ddpm':
             z_lig, z_pocket = self._graphed_joint_fast_loop(z_lig, z_pocket, lig_mask, pocket_mask, n_samples, timesteps, sampler,
                                                             eta, return_frames, out_lig, out_pocket)
-            self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
-        elif sampler != 'ddpm':
-            t_table, coef = self._fast_tables(timesteps, sampler, eta, z_lig.device)
-            h_lig, h_pocket = self._empty_history(z_lig, sampler), self._empty_history(z_pocket, sampler)
-            for s in reversed(range(0, timesteps)):
-                z_lig, z_pocket, h_lig, h_pocket = self._joint_fast_step(
-                    s, t_table[s].expand(n_samples, 1), coef[s:s + 1], z_lig, z_pocket, h_lig, h_pocket, lig_mask, pocket_mask,
-                    sampler, eta)
-                if (s * return_frames) % timesteps == 0:
-                    idx = (s * return_frames) // timesteps
-                    out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
-            self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
-        elif self._joint_use_graph(z_lig.device):
+        elif use_graph:
             stride = timesteps // return_frames       # frames are saved at s = idx * stride
             s_hi = timesteps - 1
             while s_hi >= 0:
@@ -999,17 +901,17 @@ class EnVariationalDiffusion(nn.Module):
                     z_lig, z_pocket, lig_mask, pocket_mask, n_samples, s_hi, s_hi - s_lo + 1, timesteps)
                 out_lig[s_lo // stride], out_pocket[s_lo // stride] = self.unnormalize_z(z_lig, z_pocket)
                 s_hi = s_lo - 1
-            self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         else:
+            fast = None if sampler == 'ddpm' else self._fast_tables(timesteps, sampler, eta, z_lig.device)
+            h_lig, h_pocket = self._empty_history(z_lig, sampler), self._empty_history(z_pocket, sampler)
             for s in reversed(range(0, timesteps)):
-                s_arr = torch.full((n_samples, 1), fill_value=s, device=z_lig.device)
-                t_arr = (s_arr + 1) / timesteps
-                s_arr = s_arr / timesteps
-                self._draw_at(seeded.STAGE_LOOP, s, 0, seeded.PURPOSE_REVERSE)
-                z_lig, z_pocket = self.sample_p_zs_given_zt(s_arr, t_arr, z_lig, z_pocket, lig_mask, pocket_mask)
+                t, row = self._eager_row(s, timesteps, n_samples, z_lig.device, fast)
+                z_lig, z_pocket, h_lig, h_pocket = self._joint_fast_step(s, t, row, z_lig, z_pocket, h_lig, h_pocket, lig_mask,
+                                                                         pocket_mask, sampler, eta)
                 if (s * return_frames) % timesteps == 0:
                     idx = (s * return_frames) // timesteps
                     out_lig[idx], out_pocket[idx] = self.unnormalize_z(z_lig, z_pocket)
+        self.assert_mean_zero_with_mask(torch.cat((z_lig[:, :self.n_dims], z_pocket[:, :self.n_dims])), combined_mask)
         self._draw_at(seeded.STAGE_FINAL)
         x_lig, h_lig, x_pocket, h_pocket = self.sample_p_xh_given_z0(z_lig, z_pocket, lig_mask, pocket_mask, n_samples)
         self.assert_mean_zero_with_mask(torch.cat((x_lig, x_pocket), dim=0), combined_mask)
