@@ -662,3 +662,82 @@ def sweep_operand_ranges(cfg, sd, inputs):
 def configs2_case():
     cfg = FULLATOM_COND
     return cfg, syn.synthetic_state_dict(cfg, 0), syn.synthetic_denoiser_inputs(cfg, [25] * 64, [175] * 64, seed=3)
+
+
+# bench.py's 'moad' workload (configs/moad_fullatom_cond.yml): hidden_nf 192 with the edge-type table
+MOAD_COND = FULLATOM_COND.with_(hidden_nf=192, edge_embedding_dim=8, edge_cutoff_pocket=4.0, edge_cutoff_interaction=7.0)
+
+
+def moad_case():
+    cfg = MOAD_COND
+    return cfg, syn.synthetic_state_dict(cfg, 0), syn.synthetic_denoiser_inputs(cfg, [25] * 64, [175] * 64, seed=3)
+
+
+# ---- the tensor-core kernel instances a forward launches ------------------------------------------------------------
+TC_FORMATS = ('TF32x3', 'F16x3', 'F16x1')          # TcFormat enumerators, in order (dsb_internal.cuh)
+
+
+def tc_instances(cfg, mode, det):
+    """{(kernel, COORD, FMT, H, TB, DET)} of the tensor-core kernels one forward launches, following dsb_dynamics_forward
+    and launch_tc_node_gemm / launch_tc_edge_gcl / launch_tc_edge_coord: mode bits 1 / 2 / 4 put the node GEMMs / GCL edge
+    kernel / coordinate edge kernel on wgmma, bits 8 / 16 pick the format, an edge-type table (edge_embedding_dim > 0)
+    selects TB.  The node GEMM is templated on FMT and H only: its COORD, TB and DET are None."""
+    mm = effective_mode(cfg, mode)
+    fmt = TC_FORMATS[0] if not mm & 8 else TC_FORMATS[2] if mm & 16 else TC_FORMATS[1]
+    H, tb, det = cfg.hidden_nf, bool(cfg.edge_embedding_dim), bool(det)
+    out = set()
+    if mm & 1:
+        out.add(('tc_node_gemm_kernel', None, fmt, H, None, None))
+    for bit, coord in ((2, False), (4, True)):
+        if mm & bit:
+            out.add(('tc_edge_kernel', coord, fmt, H, tb, det))
+    return out
+
+
+def _template_arg(s):
+    """One demangled template argument: '(bool)1' / 'true', '(int)192' / '192', '(dsb::TcFormat)1' / 'dsb::TcFormat::F16x3'."""
+    s = s.strip()
+    if s.startswith('('):
+        typ, val = s[1:].split(')', 1)
+        if typ == 'bool':
+            return bool(int(val))
+        if typ.endswith('TcFormat'):
+            return TC_FORMATS[int(val)]
+        return int(val)
+    if s in ('true', 'false'):
+        return s == 'true'
+    if 'TcFormat::' in s:
+        name = s.rsplit('::', 1)[1]
+        assert name in TC_FORMATS, s
+        return name
+    return int(s)
+
+
+def demangle(names):
+    """Demangled forms of kernel names (cu++filt from the CUDA toolkit; names that are not mangled pass unchanged)."""
+    names = list(names)
+    mangled = [n for n in names if n.startswith('_Z')]
+    if not mangled:
+        return names
+    import shutil
+    import subprocess
+    filt = shutil.which('cu++filt') or '/usr/local/cuda/bin/cu++filt'
+    out = subprocess.run([filt], input='\n'.join(mangled) + '\n', capture_output=True, text=True, check=True).stdout
+    table = dict(zip(mangled, out.splitlines()))
+    return [table.get(n, n) for n in names]
+
+
+def parse_tc_instance(name):
+    """(kernel, COORD, FMT, H, TB, DET) of a demangled tensor-core kernel name, None for any other kernel."""
+    for kernel in ('tc_node_gemm_kernel', 'tc_edge_kernel'):
+        i = name.find(kernel + '<')
+        if i < 0:
+            continue
+        args = [_template_arg(a) for a in name[i + len(kernel) + 1:name.index('>', i)].split(',')]
+        if kernel == 'tc_node_gemm_kernel':
+            fmt, H = args
+            return kernel, None, fmt, H, None, None
+        coord, fmt, H, tb = args[:4]
+        det = args[4] if len(args) > 4 else False        # DET = false is a default argument: it may be left out
+        return kernel, coord, fmt, H, tb, det
+    return None

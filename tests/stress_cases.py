@@ -36,7 +36,9 @@ def _ladder(n):
 #   expect: min_max_deg (largest receiver degree at least), csr_cross / virt_cross (receivers whose segment crosses a
 #   128-row boundary in CSR / virtual order: at least 1), span3 (receivers whose virtual segment touches >= 3 tiles: at
 #   least 1), min_deg_lig (every ligand atom has at least this degree), deg1 (a receiver of degree exactly 1), empty
-#   (graph ids with no node), no_pocket / no_ligand (graph ids with ligand atoms only / pocket nodes only)
+#   (graph ids with no node), no_pocket / no_ligand (graph ids with ligand atoms only / pocket nodes only), edge_types
+#   (ligand-ligand, pocket-pocket and ligand-pocket edges all present), min_units (more than this many 128-row units of
+#   the virtual edge order in the GCL and in the coordinate edge kernel)
 CASES = {
     # conditional, no cut-offs: degree = graph size for every node
     'ladder_h128': dict(cfg=DynamicsConfig(hidden_nf=128, joint_nf=32, n_layers=2, **NO_CUTOFF),
@@ -74,6 +76,14 @@ CASES = {
                                                           aggregation_method='mean'),
                                        graphs=[(1, 0), (0, 0), (0, 23), (9, 31), (0, 0)], seed=49, wseed=49,
                                        expect=dict(deg1=True, empty=[1, 4], no_pocket=[0], no_ligand=[2])),
+    # edge-type table at H=128 without the attention gate or tanh (the only tensor-core kernels that read the table at that
+    # width, and the gate = 1 / untanh'd branches of the edge epilogues); default cut-offs give all three edge types, and
+    # 60-atom ligands give both edge kernels more 128-row units than the H100's 132 SMs (~290 GCL, ~160 coordinate units)
+    'tb_noatt_notanh_h128': dict(cfg=DynamicsConfig(hidden_nf=128, joint_nf=32, n_layers=2, edge_embedding_dim=8,
+                                                    attention=False, tanh=False),
+                                 graphs=[(60, 150)] * 4, seed=57, wseed=57,
+                                 expect=dict(min_max_deg=80, csr_cross=True, virt_cross=True, edge_types=True,
+                                             min_units=132)),
 }
 
 # ligand rows [0, n) + pocket rows of the 257-node ladder graph, run alone and inside its batch

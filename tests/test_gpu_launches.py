@@ -44,7 +44,50 @@ updates).  The margin to the budgets is 1.3x on the clean side; planted defects,
   46 x in mode 7 (1.5x); the rest of the GPU suite passes with it.
 The worst-case bound (a rigorous check, not assuming round-to-nearest accumulation) stays far from the kernels (<= 0.5 of
 twice the bound, the largest on the single-rounding steps finish and post) and catches gross faults only.
-The whole file (42 tests) takes 21.5 s on that card.
+
+Three cases reach the tensor-core kernel instances the eight above never launch (tests/test_kernel_instances_cpu.py
+holds the list complete; ``test_kernel_instances_follow_the_dispatch`` checks it against the profiler): ``moad``
+(bench.py's moad workload, H = 192 with the edge-type table, 64 x (25 + 175) nodes), ``joint_fc_h192`` (H = 192 without
+the table, joint, receivers spanning three tiles) and ``tb_noatt_notanh_h128`` (the table at H = 128, no attention gate,
+no tanh).  Each has more 128-row edge units than the card has SMs, so every CTA runs the cross-unit pipeline; at H = 192
+the F16 formats run 3 chunks per unit, the only odd count.  Measured on one H100 80GB HBM3 at a 700 W power limit,
+largest value over layers and both modes, RMS ratio / max error over (2 x bound), tensor-core launches:
+
+    case                   launch   fp32           3xFP16         3xTF32
+    moad                   g1       1.00 / 0.012   2.97 / 0.003   5.50 / 0.005
+                           gcl      0.78 / 0.003   5.59 / 0.001  11.06 / 0.001
+                           g2       1.00 / 0.008   4.31 / 0.002   8.31 / 0.003
+                           g3       1.00 / 0.014   2.98 / 0.004   4.34 / 0.005
+                           g4       1.00 / 0.018   2.91 / 0.004   5.52 / 0.007
+                           coord    0.99 / 0.000   2.38 / 0.000   4.53 / 0.000
+    joint_fc_h192          g1       1.00 / 0.009   2.90 / 0.002   5.51 / 0.004
+                           gcl      0.51 / 0.000   2.28 / 0.001   4.51 / 0.001
+                           g2       2.10 / 0.004   6.45 / 0.002  12.55 / 0.003
+                           g3       1.00 / 0.011   2.89 / 0.003   5.44 / 0.004
+                           g4       1.00 / 0.012   2.87 / 0.004   5.46 / 0.005
+                           coord    0.51 / 0.000   1.41 / 0.000   2.34 / 0.000
+    tb_noatt_notanh_h128   g1       1.00 / 0.017   2.40 / 0.003   4.47 / 0.005
+                           gcl      0.74 / 0.004   3.89 / 0.002   7.97 / 0.003
+                           g2       1.96 / 0.008   6.59 / 0.002  13.01 / 0.003
+                           g3       1.00 / 0.013   2.39 / 0.003   3.29 / 0.004
+                           g4       1.00 / 0.017   2.42 / 0.005   4.51 / 0.006
+                           coord    0.98 / 0.000   2.27 / 0.000   3.29 / 0.000
+
+The other launches of these cases (prep, finish, centroid, velmean, post) stay at or below 2.56 / 0.499 in every mode.
+Width 192 sits no closer to the budgets than 128 and 256: its largest ratios, 12.55 (3xTF32) and 6.45 (3xFP16), are g2,
+about 2.5x under R.  Planted defects in those instances, each built once and then reverted:
+* H = 192, 3xFP16: the x_lo w_hi products of a tile's last chunk dropped in ``mma_chunk``: fails in mode 15 on moad and
+  joint_fc_h192, deterministic and default mode, g2 up to 935 x, g1 / g4 / g3 / coord 360-534 x, gcl 36-162 x (2-58x
+  the budget).  That defect is large enough for the whole-forward tests to catch as well: ``test_gpu_parity.py``
+  (moad_emb8_h192_l3 in 3xFP16) and ``test_gpu_stress_shapes.py`` (both joint_fc H = 192 cases, 3xFP16, ligand output
+  3.3e-4 against atol 1e-5);
+* H = 128 with the edge-type table: the table term scaled by 1 - 2^-10 in the edge kernels' operand build: fails in
+  modes 15 and 7 on tb_noatt_notanh_h128, deterministic and default mode, coord 832-856 x and gcl 404-409 x (13-53x the budget).  No
+  earlier test launches these instances;
+* attention off: a gate of 1 - 2^-12 instead of 1 in the GCL edge kernel: fails in modes 15 and 7 on
+  tb_noatt_notanh_h128, gcl 1 886-1 909 x (59-119x the budget); ``test_gpu_parity.py`` (the noatt_notanh goldens, whole
+  forward) and ``test_gpu_stress_shapes.py`` pass with it.
+The whole file (71 tests) takes 36-46 s on that card (two runs).
 """
 import ctypes as C
 import math
@@ -74,7 +117,15 @@ CASES = {
     'emb8_h256_l3': lambda: load_golden('emb8_h256_l3')[:3],
     'joint_b2_h128_l5': lambda: load_golden('joint_b2_h128_l5')[:3],
     'binade_sweep': lc.binade_sweep_case,
+    'moad': lc.moad_case,
+    'joint_fc_h192': lambda: case_inputs('joint_fc_h192'),
+    'tb_noatt_notanh_h128': lambda: case_inputs('tb_noatt_notanh_h128'),
 }
+# cases also checked in the default mode (atomic receiver sums): together with the deterministic runs they launch every
+# tensor-core kernel instance the library has (tests/test_kernel_instances_cpu.py)
+DEFAULT_MODE_CASES = ('configs2', 'ladder_h256', 'emb8_h256_l3', 'joint_b2_h128_l5', 'binade_sweep', 'moad', 'joint_fc_h192',
+                      'tb_noatt_notanh_h128')
+SYNTHETIC_CFGS = {'configs2': lc.FULLATOM_COND, 'moad': lc.MOAD_COND}     # without building their 12 800-node inputs
 RESULTS = []
 
 
@@ -194,10 +245,14 @@ class Runner:
                 self.failures.append(f'{what}: RMS error {rms_k:.3e} = {rr:.2f} x the fp32 evaluation ({rms_32:.3e})')
 
 
+def case_cfg(name):
+    return SYNTHETIC_CFGS[name] if name in SYNTHETIC_CFGS else CASES[name]()[0]
+
+
 def params():
     out = []
     for name in CASES:
-        cfg = CASES[name]()[0] if name not in ('configs2',) else lc.FULLATOM_COND
+        cfg = case_cfg(name)
         for mode in MODES:
             if lc.effective_mode(cfg, mode) == mode:
                 out.append((name, mode))
@@ -222,8 +277,10 @@ def test_launches_deterministic(name, mode):
 READS_ONLY = ('prep', 'g1', 'gcl', 'g2', 'g4', 'coord', 'centroid', 'velmean', 'post')
 
 
-@pytest.mark.parametrize('name,mode', [p for p in PARAMS if p[0] in ('configs2', 'ladder_h256', 'emb8_h256_l3',
-                                                                      'joint_b2_h128_l5', 'binade_sweep')])
+DEFAULT_PARAMS = [p for p in PARAMS if p[0] in DEFAULT_MODE_CASES]
+
+
+@pytest.mark.parametrize('name,mode', DEFAULT_PARAMS)
 def test_launches_default_mode(name, mode):
     r = Runner(name, mode, False)
     for i, j, op in lc.launch_units(r.cfg, False):
@@ -232,6 +289,31 @@ def test_launches_default_mode(name, mode):
         S = r.state(r.snapshot(j))
         r.check_unit(op, S, S)
     assert not r.failures, '\n'.join(r.failures)
+
+
+@pytest.mark.parametrize('name', list(CASES))
+def test_kernel_instances_follow_the_dispatch(name):
+    """The tensor-core kernels one forward launches, as torch.profiler records them, are exactly
+    ``launch_cases.tc_instances``: the instance ledger of tests/test_kernel_instances_cpu.py follows the real dispatch."""
+    from torch.profiler import ProfilerActivity, profile
+    cfg, sd, inp = CASES[name]()
+    x = [t.cuda() for t in inp]
+    net = make_net(cfg, sd, 0, True)
+    run_stopped(net, x, -1)
+    wrong = []
+    for mode in MODES + (31,):
+        for det in (True, False):
+            net.math_mode, net.deterministic = mode, det
+            run_stopped(net, x, -1)                    # any re-packing happens outside the trace
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                run_stopped(net, x, -1)
+            names = {e.name for e in prof.events() if 'tc_node_gemm_kernel' in e.name or 'tc_edge_kernel' in e.name}
+            got = {lc.parse_tc_instance(n) for n in lc.demangle(names)}
+            want = lc.tc_instances(cfg, mode, det)
+            if got != want:
+                wrong.append(f'mode {mode} det {int(det)}: launched {sorted(map(str, got))}, ledger {sorted(map(str, want))}'
+                             f' (names {sorted(names)})')
+    assert not wrong, f'{name}:\n' + '\n'.join(wrong)
 
 
 # workspace state each operation writes (deterministic mode; the edge kernels write the partial buffer, their segment

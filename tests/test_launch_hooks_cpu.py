@@ -81,10 +81,10 @@ def test_op_sequence_counts():
     assert units[-1][2].kind == 'velmean' and units[-1][1] == len(lc.op_sequence(FULLATOM_JOINT, True))
 
 
-EMU_CASES = ['emb8_h256_l3', 'joint_emb8_sub2_reflect_h256_l2', 'mean_h256_l3', 'joint_b2_h128_l5']
+EMU_CASES = ['emb8_h256_l3', 'joint_emb8_sub2_reflect_h256_l2', 'mean_h256_l3', 'joint_b2_h128_l5', 'moad_emb8_h192_l3']
 
 
-@pytest.mark.parametrize('name', EMU_CASES + ['degenerate_joint_mean_h128', 'sweep'])
+@pytest.mark.parametrize('name', EMU_CASES + ['degenerate_joint_mean_h128', 'joint_fc_h192', 'tb_noatt_notanh_h128', 'sweep'])
 def test_restatements_chain_to_the_oracle(name):
     if name == 'sweep':
         cfg, sd, inp = lc.binade_sweep_case()
@@ -102,7 +102,7 @@ def test_restatements_chain_to_the_oracle(name):
             assert_close(a, b, f'{name}: fp32 restatements vs fp64 oracle')
 
 
-@pytest.mark.parametrize('name', ['emb8_h256_l3', 'joint_emb8_sub2_reflect_h256_l2', 'sweep'])
+@pytest.mark.parametrize('name', ['emb8_h256_l3', 'joint_emb8_sub2_reflect_h256_l2', 'moad_emb8_h192_l3', 'sweep'])
 def test_fp32_launches_inside_their_bounds(name):
     """Teacher-forced on the fp32 chain: every launch's fp32 evaluation is within its float64 worst-case bound."""
     if name == 'sweep':

@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from helpers import assert_close, ATOL, RTOL
-from stress_cases import CASES, case_inputs, edge_stats, column_errors
+from stress_cases import CASES, CHUNK, TILE, case_inputs, edge_stats, column_errors
 from diffsbdd_b200 import synthetic as syn
 from oracle import egnn_oracle
 
@@ -37,6 +37,16 @@ def test_case_structure(name):
     if cfg.edge_cutoff_ligand is None and cfg.edge_cutoff_pocket is None and cfg.edge_cutoff_interaction is None:
         size = torch.bincount(torch.cat([ma, mr]), minlength=B)
         assert torch.equal(deg, size[torch.cat([ma, mr])])       # fully connected graphs: degree = graph size
+    if ex.get('edge_types'):
+        NL, er, ec = len(ma), edges[0], edges[1]
+        assert bool(((er < NL) & (ec < NL)).any()) and bool(((er >= NL) & (ec >= NL)).any())
+        assert bool(((er < NL) != (ec < NL)).any())
+    if 'min_units' in ex:
+        vdeg = (deg + CHUNK - 1) // CHUNK * CHUNK
+        n_coord = len(deg) if cfg.update_pocket_coords else len(ma)
+        for what, rows in (('GCL', vdeg), ('coordinate', vdeg[:n_coord])):
+            units = -(-int(rows.sum()) // TILE)
+            assert units > ex['min_units'], f'{what} edge kernel: {units} units'
     for g in ex.get('empty', []):
         assert not bool((ma == g).any()) and not bool((mr == g).any())
     for g in ex.get('no_pocket', []):
